@@ -1,4 +1,4 @@
-"""Build libaigw_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libaigw_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -6,6 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libaigw_b200.so")
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
 
 
@@ -31,7 +32,7 @@ def build(force=False, verbose=False):
     from concurrent.futures import ThreadPoolExecutor
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
-    base = [nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+    base = [nvcc()] + GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
     if verbose:
         base.insert(1, "-Xptxas=-v")
     hdr_t = max(os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) if os.listdir(CSRC) else 0
@@ -49,7 +50,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(len(SOURCES), os.cpu_count() or 2)) as ex:
         objs = list(ex.map(one, SOURCES))
-    subprocess.check_call([nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-o", SO] + objs)
+    subprocess.check_call([nvcc()] + GENCODE + ["-shared", "-cudart", "static", "-o", SO] + objs)
     return SO
 
 

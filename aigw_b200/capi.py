@@ -178,7 +178,7 @@ class Context:
         h = C.c_void_p()
         rc = self.L.aigw_init(device, C.byref(h))
         if rc != 0 or not h.value:
-            raise RuntimeError(f"aigw_init(device={device}) failed with CUDA error {rc}: this library needs a B200 (sm_100a); there is no CPU path")
+            raise RuntimeError(f"aigw_init(device={device}) failed with CUDA error {rc}: this library needs an H100 (sm_90a); there is no CPU path")
         self.h = h
         self.sm_count = self.L.aigw_device_sm_count(self.h)
 

@@ -1,4 +1,4 @@
-// See bedrock_stream_kernel.cuh.  sm_100a only.
+// See bedrock_stream_kernel.cuh.  sm_90a only.
 #include <cstring>
 
 #include "bedrock_common.cuh"

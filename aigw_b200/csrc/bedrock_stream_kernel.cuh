@@ -1,4 +1,4 @@
-// aigw_b200 — Bedrock ConverseStream (AWS eventstream) → OpenAI SSE back-translation (S2) for sm_100a.
+// aigw_b200 — Bedrock ConverseStream (AWS eventstream) → OpenAI SSE back-translation (S2) for sm_90a.
 //
 // Replaces openAIToAWSBedrockTranslatorV1ChatCompletion.ResponseBody for streamed responses
 // (internal/translator/openai_awsbedrock.go:695-732), extractAmazonEventStreamEvents (:829-852),

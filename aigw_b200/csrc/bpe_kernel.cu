@@ -11,7 +11,7 @@
 // them into symbol ids, finds the piece starts with ballots, and then every LANE runs the merge loop of one piece at a time
 // (pieces are independent).  Per piece the ranks of the adjacent pairs are kept next to the symbols, so a merge costs two
 // table lookups and one shift instead of a rescan.  A text longer than the buffer is cut at piece boundaries; a single piece
-// longer than the buffer is DECLINED (count 0xFFFFFFFF) rather than approximated.  sm_100a only.
+// longer than the buffer is DECLINED (count 0xFFFFFFFF) rather than approximated.  sm_90a only.
 #include "bpe_kernel.cuh"
 
 #include <cstdio>

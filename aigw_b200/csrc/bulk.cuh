@@ -1,4 +1,4 @@
-// 1-D bulk asynchronous copies (the TMA engine without a tensor map) + mbarrier completion, sm_100a.
+// 1-D bulk asynchronous copies (the TMA engine without a tensor map) + mbarrier completion, sm_90a.
 // A warp stages one request body with ONE instruction issued by one lane: the copy costs no load/store
 // issue slots in kernels that are issue-bound, and the bytes land while the warp does other work.
 //   cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes  → SASS UBLKCP

@@ -1,4 +1,4 @@
-// aigw_b200 — CEL cost expressions as device bytecode (C2 / SURVEY §8f rank 2), sm_100a.
+// aigw_b200 — CEL cost expressions as device bytecode (C2 / SURVEY §8f rank 2), sm_90a.
 //
 // Replaces llmcostcel.NewProgram / EvaluateProgram (internal/llmcostcel/cel.go:55-99) as evalCost calls them per request at
 // end of stream (internal/extproc/processor_impl.go:728-751) for the typed subset that cost expressions use: the three string

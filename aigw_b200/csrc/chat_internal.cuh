@@ -1,7 +1,6 @@
-// See chat_kernel.cuh for the design.  sm_100a only.
+// See chat_kernel.cuh for the design.  sm_90a only.
 //
-// v2 layout of the work (driven by profiles/r01_chat_v1.md: 72 % of v1's time was single-lane
-// sequential code at ~22 cycles per instruction):
+// v2 layout of the work (v1 spent most of its time in single-lane sequential code):
 //   * tokens carry their byte (tty) and a precomputed key / value id (tkid) that 32 lanes compute in
 //     parallel, so the schema walk compares one byte instead of strings;
 //   * the copy-op under construction lives in registers; shared memory is touched once per finished op;
@@ -270,6 +269,6 @@ __host__ __device__ inline WorkPtrs carve(uint8_t* base, size_t ndocs, const Wor
 }
 
 // K2 (chat_walk.cu): validate + schema walk, one thread per document of the sub-batch
-cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, const WorkLayout& layout, cudaStream_t st, int blocks_per_sm = 0);   // 0: AIGW_WALK_BLOCKS
+cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, const WorkLayout& layout, cudaStream_t st, int blocks_per_sm = 0);   // 0: the default (chat_walk.cu)
 
 }  // namespace aigw

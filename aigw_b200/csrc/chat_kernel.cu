@@ -1,5 +1,5 @@
 // Index (K1), sort (Ks) and emit (K3) stages of the chat translate pass + the launcher.  See chat_kernel.cuh for the design;
-// the schema walk (K2) is in chat_walk.cu.  sm_100a only.
+// the schema walk (K2) is in chat_walk.cu.  sm_90a only.
 //
 //   * tokens carry their byte (tty) and a precomputed key / value id (tkid) that 32 lanes compute in
 //     parallel, so the schema walk compares one byte instead of strings;
@@ -220,11 +220,11 @@ size_t work_bytes_cls(size_t ndocs) { return work_per_doc(layout_of<MAXD>()) * n
 
 struct ClsConfig { bool ready = false; int bps1 = 1, bps3 = 1; };
 
-// documents per sub-batch: the bodies of the sub-batches in flight (two streams) stay in the 126 MB L2 between index and emit
+// documents per sub-batch: the bodies of the sub-batches in flight (two streams) stay in the 50 MB L2 between index and emit
 static size_t sub_batch_docs(int maxd) {
   static const long env = getenv("AIGW_CHAT_SUB") ? atol(getenv("AIGW_CHAT_SUB")) : 0;
   if (env > 0) return (size_t)env;
-  size_t d = ((size_t)40 << 20) / (size_t)maxd;
+  size_t d = ((size_t)20 << 20) / (size_t)maxd;
   size_t p = 256; while (p * 2 <= d) p *= 2;
   return p;
 }
@@ -264,7 +264,7 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
   static const int env_pipe = getenv("AIGW_CHAT_PIPE") ? atoi(getenv("AIGW_CHAT_PIPE")) : 0;
   // ---- stage-pipelined mode: one stream per STAGE, sub-batches flow index -> walk -> emit through a ring of workspaces, so in
   // the steady state one index, one walk and one emit kernel (of three consecutive sub-batches) are resident on every SM at
-  // once.  The walk is latency-bound (IPC 0.4) while index and emit are bound by the integer issue rate, so sharing an SM costs
+  // once.  The walk is latency-bound while index and emit are bound by the integer issue rate, so sharing an SM costs
   // each little; every kernel's grid is capped so that the three fit together (registers: 3x128x80 + 2x128x54 + 2x128x56).
   if (env_pipe && aux && !ev && P.n > 4096) {
     const int ic = env_idx_ctas > 0 ? env_idx_ctas : 2, wc = env_walk_ctas > 0 ? env_walk_ctas : 3, ec = env_emit_ctas > 0 ? env_emit_ctas : 2;

@@ -1,4 +1,4 @@
-// aigw_b200 — /v1/chat/completions parse + translate kernel for sm_100a.
+// aigw_b200 — /v1/chat/completions parse + translate kernel for sm_90a.
 //
 // One warp per request body ("document"), persistent CTAs pulling documents from a global
 // counter.  Per document:

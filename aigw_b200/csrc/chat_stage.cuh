@@ -1,5 +1,5 @@
 // Per-document stage bodies of the chat translate pass, shared by the persistent throughput kernels (chat_kernel.cu) and the
-// fused small-batch kernel (chat_walk_impl.cuh): index_doc (stages 2 + 2.5), emit_prefix / emit_doc (stage 5).  sm_100a only.
+// fused small-batch kernel (chat_walk_impl.cuh): index_doc (stages 2 + 2.5), emit_prefix / emit_doc (stage 5).  sm_90a only.
 #pragma once
 #include "chat_internal.cuh"
 #include "classify.cuh"

@@ -12,12 +12,18 @@ AIGW_WALK_DECL(0) AIGW_WALK_DECL(1) AIGW_WALK_DECL(2) AIGW_WALK_DECL(3) AIGW_WAL
 AIGW_SMALL_DECL(0) AIGW_SMALL_DECL(1) AIGW_SMALL_DECL(2) AIGW_SMALL_DECL(3) AIGW_SMALL_DECL(4) AIGW_SMALL_DECL(5) AIGW_SMALL_DECL(6) AIGW_SMALL_DECL(7) AIGW_SMALL_DECL(8) AIGW_SMALL_DECL(9)
 #undef AIGW_SMALL_DECL
 
+// resident walk blocks per SM.  The launch bound keeps room for AIGW_WALK_BLOCKS (the register budget), but the walk is bound by
+// L1 / L2 behaviour of its per-thread token lists and fewer warps run faster.  On an H100 80GB HBM3 at a 400 W power limit, walk
+// time per 1 M 4 KB bodies (bench.py config 2, the settings alternated within each of three runs of the bench): 4.13-4.17 ms at
+// 3 blocks over 9 runs, 4.35-4.37 ms at 4 blocks over 7 runs, 4.27-4.28 ms at 2 blocks over 2 runs.
+constexpr int kWalkBlocksPerSm = 3;
+
 cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, const WorkLayout& layout, cudaStream_t st, int blocks_per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
-  { static int sm_cache[kMaxDevices] = {0}; if (dev >= 0 && dev < kMaxDevices) { if (!sm_cache[dev]) cudaDeviceGetAttribute(&sm_cache[dev], cudaDevAttrMultiProcessorCount, dev); sms = sm_cache[dev] ? sm_cache[dev] : 148; } }
-  static const int env_ctas = getenv("AIGW_WALK_CTAS") ? atoi(getenv("AIGW_WALK_CTAS")) : 0;   // experiment: fewer resident blocks per SM (room for the other stages' blocks)
-  if (blocks_per_sm <= 0 || blocks_per_sm > AIGW_WALK_BLOCKS) blocks_per_sm = env_ctas > 0 && env_ctas < AIGW_WALK_BLOCKS ? env_ctas : AIGW_WALK_BLOCKS;
+  { static int sm_cache[kMaxDevices] = {0}; if (dev >= 0 && dev < kMaxDevices) { if (!sm_cache[dev]) cudaDeviceGetAttribute(&sm_cache[dev], cudaDevAttrMultiProcessorCount, dev); sms = sm_cache[dev] ? sm_cache[dev] : 132; } }
+  static const int env_ctas = getenv("AIGW_WALK_CTAS") ? atoi(getenv("AIGW_WALK_CTAS")) : 0;   // experiment: another number of resident blocks per SM
+  if (blocks_per_sm <= 0 || blocks_per_sm > AIGW_WALK_BLOCKS) blocks_per_sm = env_ctas > 0 && env_ctas <= AIGW_WALK_BLOCKS ? env_ctas : kWalkBlocksPerSm;
   sms *= blocks_per_sm;
   const uint32_t s = P.schema;
   if (s & (uint32_t)AIGW_SCHEMA_MESSAGES)   // the full re-maps (OpenAI / Bedrock targets) have their own kernel

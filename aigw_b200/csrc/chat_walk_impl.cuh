@@ -1,13 +1,12 @@
 // K2 of the chat translate pass: JSON grammar + bracket matching over the token list, then the schema walk that plans the
 // output as copy ops.  One thread per document; compiled once for every size class (slot sizes are kernel arguments).
-// See chat_kernel.cuh for the design and chat_kernel.cu for the index / emit stages.  sm_100a only.
+// See chat_kernel.cuh for the design and chat_kernel.cu for the index / emit stages.  sm_90a only.
 //
 // This file is the body of two translation units per schema group (chat_walk_g*.cu: the throughput walk kernel;
 // chat_small_g*.cu, which also define AIGW_WALK_SMALL: the fused small-batch kernel — one kernel per unit, so that every
 // planner has a single call site and is inlined with the Walker in registers).  They define AIGW_WALK_GROUP and include it: a
 // kernel that carries only its own planner keeps its code and its stack frame small, which is what a latency-bound
-// thread-per-document kernel pays for (measured on B200: the Bedrock walk went 2.95 -> 3.65 ms per 1 M bodies when the
-// Anthropic-response and Gemini planners were added to the single kernel).
+// thread-per-document kernel pays for (the Bedrock walk slowed by a quarter when the Anthropic-response and Gemini planners were added to the single kernel).
 #pragma once
 #ifndef AIGW_WALK_GROUP
 #error "include from chat_walk_g*.cu with AIGW_WALK_GROUP defined"

@@ -1,7 +1,7 @@
 // BASELINE config 3: large /v1/embeddings requests (1024 inputs of 64 characters, about 68.7 KB of JSON, above the 64 KiB
 // ceiling of the warp-per-document translate pass) — EmbeddingsEndpointSpec.ParseBody (internal/endpointspec/endpointspec.go:231-240)
 // over the input union's []string / string forms (internal/apischema/openai/union.go:71-147, openai.go:316-375) fused with the
-// text table the BPE count kernel (bpe_kernel.cu) reads IN PLACE from the request bytes.  sm_100a only.
+// text table the BPE count kernel (bpe_kernel.cu) reads IN PLACE from the request bytes.  sm_90a only.
 //
 // Mapping: one CTA of 256 threads per request, persistent CTAs pulling requests from a counter; the body streams through in
 // 8 KB tiles (32 bytes per thread, two coalesced 16-byte loads), nothing of it is kept on chip:

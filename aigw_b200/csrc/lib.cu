@@ -155,7 +155,7 @@ cudaError_t chat_small_launch(const aigw_backend_cfg* cfg, const uint8_t* in, co
 // host loops over the calls of one window (byte staging, result hand-back) run on a few threads when the window is large
 template <class F>
 static void host_parallel_for(uint32_t n, F&& f) {
-  static const unsigned hw = [] { unsigned h = 2; const char* e = getenv("AIGW_HOST_THREADS"); if (e) h = (unsigned)atoi(e); return h < 1 ? 1u : (h > 8 ? 8u : h); }();   // measured: more staging threads slow the DMA that follows (17.3 / 20.0 / 19.5 / 15.9 M chunks/s at 1 / 2 / 4 / 8)
+  static const unsigned hw = [] { unsigned h = 2; const char* e = getenv("AIGW_HOST_THREADS"); if (e) h = (unsigned)atoi(e); return h < 1 ? 1u : (h > 8 ? 8u : h); }();   // more staging threads slow the DMA that follows
   if (n < 16384 || hw == 1) { f(0u, n); return; }
   std::vector<std::thread> th;
   const uint32_t per = (n + hw - 1) / hw;
@@ -166,7 +166,7 @@ static void host_parallel_for(uint32_t n, F&& f) {
 
 extern "C" {
 
-const char* aigw_version(void) { return "aigw_b200 0.1 (sm_100a)"; }
+const char* aigw_version(void) { return "aigw_b200 0.1 (sm_90a)"; }
 
 int aigw_init(int device, aigw_ctx** out) {
   *out = nullptr;
@@ -180,7 +180,8 @@ int aigw_init(int device, aigw_ctx** out) {
   e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) { (void)cudaGetLastError(); delete ctx; return (int)e; }
   ctx->sm_count = prop.multiProcessorCount;
-  if (prop.major < 10) { fprintf(stderr, "aigw_init: device %d is sm_%d%d; this library is built for sm_100a only\n", device, prop.major, prop.minor); delete ctx; return (int)cudaErrorNoKernelImageForDevice; }
+  // sm_90a code runs on compute capability 9.0 and nothing else (architecture-specific features are not forward compatible)
+  if (prop.major != 9 || prop.minor != 0) { fprintf(stderr, "aigw_init: device %d is sm_%d%d; this library is built for sm_90a (H100) only\n", device, prop.major, prop.minor); delete ctx; return (int)cudaErrorNoKernelImageForDevice; }
   // every allocation is checked on its own: a half-built context is destroyed, never returned
   auto fail = [&](const char* what, cudaError_t err) { fprintf(stderr, "aigw_init: %s: %s\n", what, cudaGetErrorString(err)); aigw_destroy(ctx); return (int)err; };
 #define INIT_CK(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return fail(#x, _e); } while (0)

@@ -1,4 +1,4 @@
-// See mutate_kernel.cuh.  sm_100a only.
+// See mutate_kernel.cuh.  sm_90a only.
 #include "device_once.cuh"
 #include "mutate_kernel.cuh"
 

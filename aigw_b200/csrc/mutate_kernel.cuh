@@ -1,4 +1,4 @@
-// aigw_b200 — route/backend body mutation (B1) for sm_100a.
+// aigw_b200 — route/backend body mutation (B1) for sm_90a.
 //
 // Replaces BodyMutator.Mutate (internal/bodymutator/body_mutator.go:77-119) as applied by applyBodyMutation
 // (internal/extproc/util.go:107-131) to the translated request body, or to the original one when the translator left it

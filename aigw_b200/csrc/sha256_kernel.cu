@@ -1,4 +1,4 @@
-// aigw_b200 — SHA-256 of translated bodies for SigV4 (SURVEY §8f rank 1), sm_100a.
+// aigw_b200 — SHA-256 of translated bodies for SigV4 (SURVEY §8f rank 1), sm_90a.
 //
 // Replaces `payloadHash := sha256.Sum256(body)` in the AWS request signer (internal/backendauth/aws.go:93-117), which today
 // rescans every Bedrock-bound body on the CPU right after the translator produced it.  SHA-256 is sequential inside one message

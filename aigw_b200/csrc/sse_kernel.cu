@@ -1,4 +1,4 @@
-// See sse_kernel.cuh.  sm_100a only.
+// See sse_kernel.cuh.  sm_90a only.
 #include <cstring>
 #include <vector>
 

@@ -1,4 +1,4 @@
-// aigw_b200 — OpenAI SSE usage scan (S1) for sm_100a.
+// aigw_b200 — OpenAI SSE usage scan (S1) for sm_90a.
 //
 // Replaces openAIToOpenAITranslatorV1ChatCompletion.ResponseBody (stream) →
 // extractUsageFromBufferEvent (internal/translator/openai_openai.go:131-145,179-215) plus the

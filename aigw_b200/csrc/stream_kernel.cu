@@ -1,4 +1,4 @@
-// See stream_kernel.cuh.  sm_100a only.
+// See stream_kernel.cuh.  sm_90a only.
 #include <cstddef>
 #include <cstring>
 

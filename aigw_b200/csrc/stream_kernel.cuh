@@ -1,4 +1,4 @@
-// aigw_b200 — stateful per-chunk response streams (SURVEY §8b: aigw_stream_open / chunk / close), sm_100a.
+// aigw_b200 — stateful per-chunk response streams (SURVEY §8b: aigw_stream_open / chunk / close), sm_90a.
 //
 // The reference calls Translator.ResponseBody(headers, body, endOfStream) once per upstream chunk and carries only the
 // undecoded tail between calls (internal/translator/translator.go:41-76; openai_openai.go:131-145,179-193 partial line;

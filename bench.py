@@ -2,7 +2,7 @@
 """bench.py — BASELINE.json's metric.  `--config` selects the BASELINE config (default 2, the one the metric is quoted on):
 
   1  128 OpenAI ChatCompletion bodies (2 KB, 4 messages): passthrough translate + usage count, per-call latency shape
-  2  1 M OpenAI→AWS Bedrock Converse body translate, 4 KB bodies, per GPU                      (headline; the driver's run)
+  2  1 M OpenAI→AWS Bedrock Converse body translate, 4 KB bodies, per GPU                      (headline)
   4  SSE streamed response parse through the per-chunk stream ABI: streams x 256 chunks x 80 B, usage extract
   5  mixed-provider fan-out: OpenAI / Gemini / Anthropic / Bedrock translate, Zipf(1.2) body size 1-64 KB, requests routed to
      a device by hash64(request-id) % n_gpus
@@ -15,13 +15,17 @@ One step = one pass of the hot path over a batch of synthetic bodies.  Printed (
   roofline   HBM roofline of the translate pass: algorithmic bytes (input + output) ÷ CUDA-event duration vs MEASURED_PEAKS.json
   cpu_baseline  the oracle (CPU restatement of the reference Go path) on this box's host cores, bounded sample, rank 0 / N=1
 --impl reference times the CPU restatement alone on the same config (the reference is Go; no Go toolchain exists in the image).
+--dump-outputs DIR (config 2) writes what the last timed step returned to its caller as DIR/*.npy, so that two builds can be
+compared output for output on the same seeded inputs.
 """
 import argparse
 import ctypes as C
 import json
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -43,44 +47,37 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic():
-    """DRAM read+write bytes per body of the three stages, from the committed ncu --set full capture of this round
-    (profiles/r02_traffic.json, written by tools/ncu_traffic.py from gpurun_out/*.ncu-rep); None when absent."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return None
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def batcher_block():
     """The per-request path under concurrency: tools/batcher_load.cpp (C++ threads standing in for goroutines behind cgo) drives
     aigw_batcher_translate with the bodies of the workload; callers, req/s and latency percentiles per setting."""
+    tmp = tempfile.mkdtemp(prefix="aigw_bench_")   # the tree may be read-only: the load tool and its inputs live here
     try:
         import _workload as W
-        exe = "/tmp/aigw_batcher_load"
+        exe, bodies_bin, offs_bin = (os.path.join(tmp, f) for f in ("aigw_batcher_load", "bodies.bin", "offs.u64"))
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tools", "batcher_load.cpp"), "-L", os.path.join(ROOT, "aigw_b200"),
                                "-laigw_b200", "-Wl,-rpath," + os.path.join(ROOT, "aigw_b200"), "-lpthread", "-o", exe])
         ar, of, le = W.chat_corpus(2, 0, 8000)
         packed = b"".join(bytes(ar[int(of[i]):int(of[i]) + int(le[i])]) for i in range(8000))
         po = np.zeros(8001, dtype=np.uint64); np.cumsum(le[:8000], out=po[1:])
-        open("/tmp/aigw_bl_bodies.bin", "wb").write(packed); open("/tmp/aigw_bl_offs.u64", "wb").write(po.tobytes())
+        open(bodies_bin, "wb").write(packed); open(offs_bin, "wb").write(po.tobytes())
         rows = []
         for threads, reqs, mb, win in ((1, 2000, 1, 0), (64, 1000, 64, 20), (256, 800, 256, 40), (512, 600, 512, 50)):
-            out = subprocess.check_output([exe, "/tmp/aigw_bl_bodies.bin", "/tmp/aigw_bl_offs.u64", "8000", str(threads), str(reqs), str(mb), str(win)], timeout=120).decode()
+            out = subprocess.check_output([exe, bodies_bin, offs_bin, "8000", str(threads), str(reqs), str(mb), str(win)], timeout=120).decode()
             d = json.loads(out.strip().split("\n")[-1])
             rows.append({"callers": threads, "max_batch": mb, "window_us": win, "req_per_s": d["requests_per_s"], "p50_us": d["p50_us"], "p99_us": d["p99_us"], "mean_batch": d["mean_batch"],
                          "ok": d["ok"], "declined": d["declined"], "failed": d["failed"]})
         return {"tool": "tools/batcher_load.cpp (closed loop: every caller submits its next request when the previous one returns)", "rows": rows}
     except Exception as e:  # the bench line must not depend on a side tool
         return {"error": str(e)[:200]}
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region, and the card's name and power limit (part of every number)."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -115,7 +112,13 @@ class ClockSampler:
             except Exception:
                 continue
         busy = sorted(sm)[len(sm) // 2:] if sm else []  # upper half ≈ samples under load
-        return {"sm_mhz": float(np.median(busy)) if busy else None, "sm_max_mhz": mx or None, "reasons": sorted(reasons), "samples": len(sm)}
+        gpu = power_limit = None
+        try:
+            gpu, power_limit = [x.strip() for x in subprocess.check_output(["nvidia-smi", f"--id={self.index}", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                                                                            text=True, stderr=subprocess.DEVNULL, timeout=30).strip().split(",")]
+        except Exception:
+            pass
+        return {"sm_mhz": float(np.median(busy)) if busy else None, "sm_max_mhz": mx or None, "reasons": sorted(reasons), "samples": len(sm), "gpu": gpu, "power_limit_w": power_limit}
 
 
 def host_cores():
@@ -178,6 +181,37 @@ def run_reference(a, ncpu):
 
 
 # ------------------------------------------------------------------------------------------------ config 2 (headline)
+RESULT_FIELDS = ("status", "reason", "body_len", "path_len", "body_kind", "flags", "model_off", "model_len")
+
+
+def dump_outputs2(out_dir, ctx, res, d_out, max_rows=1 << 20, max_record_bytes=4 << 20, n_records=512):
+    """What the last timed step handed its caller, as float arrays (at most 57 MB): every field of the result table but out_off
+    (<field>.npy, for the rows in result_index.npy: all of them up to max_rows, else a seeded sample), and the produced
+    records (":path" + body bytes, concatenated in record_bytes.npy, lengths in record_len.npy) of a seeded sample of the
+    accepted bodies (record_index.npy).  out_off is left out: the device bump allocator places the records in completion
+    order, so it changes from run to run while the bytes it points at do not."""
+    import aigw_b200 as A
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(res)
+    rows = np.arange(n) if n <= max_rows else np.sort(np.random.default_rng(0).choice(n, max_rows, replace=False))
+    np.save(os.path.join(out_dir, "result_index.npy"), rows.astype(np.float64))
+    for f in RESULT_FIELDS:
+        np.save(os.path.join(out_dir, f + ".npy"), res[f][rows].astype(np.float32))
+    ok = np.nonzero(res["status"] == A.AIGW_OK)[0]
+    idx, recs, budget = [], [], max_record_bytes
+    for i in np.sort(np.random.default_rng(1).permutation(ok)[:n_records]):
+        ln = int(res["path_len"][i]) + int(res["body_len"][i])
+        if ln > budget:
+            break
+        rec = np.zeros(ln, dtype=np.uint8)
+        if ln:
+            ctx.d2h(rec, d_out + int(res["out_off"][i]))
+        idx.append(int(i)); recs.append(rec); budget -= ln
+    np.save(os.path.join(out_dir, "record_index.npy"), np.asarray(idx, dtype=np.float64))
+    np.save(os.path.join(out_dir, "record_len.npy"), np.asarray([len(r) for r in recs], dtype=np.float64))
+    np.save(os.path.join(out_dir, "record_bytes.npy"), (np.concatenate(recs) if recs else np.zeros(0, np.uint8)).astype(np.float32))
+
+
 def escaped_corpus(arena, offs, lens, count):
     """accept-rate corpus: the first `count` workload bodies, every tenth re-serialised the way ASCII-only JSON encoders write them
     (non-ASCII characters as \\uXXXX, slashes escaped in half of those)"""
@@ -254,6 +288,8 @@ def run_config2(a, rank, world, local, ncpu):
     wall = time.perf_counter() - t0
     dev_s = float(np.sum(kms)) / 1e3
     res = np.zeros(n, dtype=A.DocResult); ctx.d2h(res, d_res)
+    if a.dump_outputs and rank == 0:
+        dump_outputs2(a.dump_outputs, ctx, res, d_out)
     n_ok = int((res["status"] == A.AIGW_OK).sum())
     out_bytes = int(res["body_len"].astype(np.uint64).sum() + res["path_len"].astype(np.uint64).sum())
     alg_bytes = int(lens.astype(np.uint64).sum()) + out_bytes  # SURVEY.md §8d: bytes_in + bytes_out per body
@@ -271,8 +307,8 @@ def run_config2(a, rank, world, local, ncpu):
         WL = W.lib()
         # The copies in and out model the shim's goroutines.  Default: one call over the whole step (copy in, call, copy out).  With
         # --e2e-lanes L --e2e-parts P the step is cut into P sub-batches dealt to L host threads, each with its own context on this GPU
-        # (one device call in flight per context), so that one lane copies while the other waits on the GPU — measured slower than the
-        # single call (sub-batches lose the call's internal H2D / kernel / D2H overlap; see DESIGN.md §4.6).  Either way every byte goes
+        # (one device call in flight per context), so that one lane copies while the other waits on the GPU (sub-batches lose
+        # the call's internal H2D / kernel / D2H overlap; see DESIGN.md §4.6).  Either way every byte goes
         # arena <- caller memory, H2D, kernels, D2H, caller memory <- arena inside the timed region.
         import threading
         parts = max(1, a.e2e_parts); lanes = max(1, min(a.e2e_lanes, parts))
@@ -368,18 +404,16 @@ def run_config2(a, rank, world, local, ncpu):
         peak, peak_src = hbm_peak()
         step_s = dev_s_max / a.steps
         achieved = alg_bytes / (dev_s / a.steps) / 1e9
-        tr = ncu_traffic()
         cfgd = config2_dict(n)
         detail = {}
         detail.update({"mean_in_bytes": float(lens.mean()), "mean_out_bytes": out_bytes / max(1, n_ok), "accepted": n_ok, "declined": n - n_ok,
-                     "l2": f"inputs larger than L2 ({in_bytes / 1e6:.0f} MB in + {out_bytes / 1e6:.0f} MB out per step vs 126 MB L2)",
+                     "l2": f"inputs larger than L2 ({in_bytes / 1e6:.0f} MB in + {out_bytes / 1e6:.0f} MB out per step vs 50 MB L2)",
                      "wall_ms_per_step_incl_launch": wall_max / a.steps * 1e3, "numa_node": node, "host_threads": ncpu_local})
         line = {"metric": METRIC, "value": tot_bodies / step_s, "unit": "bodies/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
                 "ms_per_step": step_s * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
                 "config": cfgd, "config_detail": detail,
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "traffic": (tr["bytes_per_body"] * n) if tr else None, "peak_source": peak_src,
-                             "traffic_source": (tr["source"] if tr else "no ncu capture committed for this round"),
+                             "traffic": None, "peak_source": peak_src, "traffic_source": "not measured",
                              "kernel": "chat_index_kernel + chat_walk_kernel + chat_emit_kernel (the three stages of one translate pass)",
                              "algorithmic_bytes_per_step": alg_bytes, "avg_step_ms": dev_s / a.steps * 1e3,
                              "stage_ms_profiled_pass": {"index": stage[0], "walk": stage[1], "emit": stage[2], "sum": serial_ms},
@@ -421,7 +455,7 @@ def run_config1(a, local, ncpu):
     from aigw_b200 import capi
     ra, ro, rl = capi.pack_bodies(resp)
     lat = []
-    for k in range(a.warmup + a.steps * 20):
+    for k in range(a.warmup + a.steps):
         t = time.perf_counter()
         res, out, st = ctx.chat_translate_host(cfg, pin, offs[:128].copy(), lens)
         ru = ctx.response_usage_host(ra, ro, rl)
@@ -537,7 +571,7 @@ def run_config3(a, rank, world, local, ncpu):
                 "ms_per_step": step_s * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8/u16", "data": "synthetic",
                 "config": {"workload": f"configs[2]: {nreq} /v1/embeddings requests per GPU per step, each a {blen}-byte JSON body with 1024 inputs x 64 characters (Zipf words, seed 3): ParseBody (request scan) + BPE count of every input "
                                        f"(vocabulary of {vocab['vocab_size']}, tests/golden/bpe_vocab.json) + per-request sums",
-                           "inputs_per_step": nt, "l2": f"requests larger than L2 ({nbytes / 1e6:.0f} MB per step vs 126 MB)", "mean_tokens_per_request": float(res["tokens"].mean()),
+                           "inputs_per_step": nt, "l2": f"requests larger than L2 ({nbytes / 1e6:.0f} MB per step vs 50 MB)", "mean_tokens_per_request": float(res["tokens"].mean()),
                            "requests_checked_vs_cpu_restatement": checked, "wall_ms_per_step": wall / a.steps * 1e3},
                 "stage_ms_per_step": {"emb_scan_kernel": stage[0] / a.steps, "bpe_count_kernel": stage[1] / a.steps, "emb_sum_kernel": stage[2] / a.steps, "whole_call_incl_readback": stage[3] / a.steps},
                 "roofline": {"bound": "hbm", "achieved": alg / step_s / 1e9, "peak": peak, "unit": "GB/s", "frac": alg / step_s / 1e9 / peak, "traffic": None, "peak_source": peak_src, "kernel": "emb_scan_kernel + bpe_count_kernel",
@@ -720,9 +754,14 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--cpu-sample", type=int, default=400_000)
     ap.add_argument("--skip-e2e", action="store_true")
-    ap.add_argument("--e2e-lanes", type=int, default=1, help="config 2 e2e: host threads (each with its own context) keeping a call in flight; measured: 2 lanes x 8 sub-batches 4.81 M bodies/s vs 5.23 M for one call over the whole step (the call's own H2D / kernel / D2H pipeline is what counts)")
+    ap.add_argument("--e2e-lanes", type=int, default=1, help="config 2 e2e: host threads (each with its own context) keeping a call in flight")
     ap.add_argument("--e2e-parts", type=int, default=1, help="config 2 e2e: sub-batches per step, dealt to the lanes round robin")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="config 2: write what the last timed step computed as DIR/<name>.npy (float32 / float64, at most 64 MB)")
     a = ap.parse_args()
+    if a.dump_outputs and (a.config != 2 or a.impl != "b200"):
+        ap.error("--dump-outputs is implemented for the product arm of config 2")
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1)); local = int(os.environ.get("LOCAL_RANK", 0))
     ncpu = host_cores()
     if a.bodies <= 0:

@@ -1,5 +1,5 @@
 /*
- * aigw_b200 — C ABI of the B200-native ext_proc body pipeline.
+ * aigw_b200 — C ABI of the H100-native ext_proc body pipeline.
  *
  * This is the drop-in boundary (SURVEY.md §8b): the entry points a cgo shim inside the reference's
  * Go extproc would bind.  Plain pointers and sizes only; no Go pointer is retained after a call

@@ -32,7 +32,7 @@ namespace oracle { TranslateResult gemini_request_body(const ChatReq& r, const s
 using namespace oracle;
 
 // The batch helpers run one worker per host thread.  glibc's defaults return freed memory to the kernel and map large blocks
-// eagerly, which serialises 128 workers on the process's mm lock (observed: 0.4–2.0 M bodies/s run to run on the bench box);
+// eagerly, which serialises 128 workers on the process's mm lock (the rate then varies widely from run to run);
 // keeping freed memory in the arenas makes the CPU baseline both faster and repeatable — closer to Go's per-P allocator caches.
 __attribute__((constructor)) static void oracle_tune_allocator() {
   if (getenv("ORACLE_NO_MALLOPT")) return;

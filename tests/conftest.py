@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     # the oracle is test infrastructure: build it on demand for the CPU suite
     so = os.path.join(ROOT, "oracle", "liboracle.so")
     if not os.path.exists(so):

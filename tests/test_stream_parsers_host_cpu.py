@@ -1,7 +1,7 @@
 """CPU-only pre-check of the per-thread stream parsers: tools/stream_host_check.cpp compiles the step functions of
 aigw_b200/csrc/stream_kernel.cu for the host (test tooling — the product has no CPU path and never links this) and
 tools/stream_host_check.py runs the GPU tests' goldens and corpora through them against the oracle.  What passes here has so far passed
-unchanged on the B200; the GPU tests remain the parity tests proper."""
+unchanged on the GPU; the GPU tests remain the parity tests proper."""
 import importlib.util
 import os
 import shutil

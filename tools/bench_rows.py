@@ -20,7 +20,7 @@ a = ap.parse_args()
 ctx = A.Context(0)
 from bench import host_cores
 ncpu = host_cores()   # affinity mask ∩ cgroup CPU quota
-peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
 L = O.lib()
 
 

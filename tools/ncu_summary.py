@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Summarise an .ncu-rep (read here, no GPU needed) and a launch-list CSV into markdown for profiles/.
+"""Summarise an .ncu-rep (read here, no GPU needed) and a launch-list CSV into markdown.
 usage: tools/ncu_summary.py <report.ncu-rep> [launches.csv]"""
 import csv, io, subprocess, sys, collections
 

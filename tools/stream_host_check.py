@@ -5,8 +5,10 @@ import importlib.util
 import json
 import os
 import random
+import shutil
 import subprocess
 import sys
+import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests")); sys.path.insert(0, ROOT)
@@ -20,10 +22,24 @@ def load(name):
 
 
 class Host:
+    """The host build of the parsers as a child process; use it as a context manager, which removes the build when it ends."""
+
     def __init__(self):
-        exe = "/tmp/stream_host_check"
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-I/usr/local/cuda/include", "-o", exe, os.path.join(ROOT, "tools", "stream_host_check.cpp")], stderr=subprocess.DEVNULL)
-        self.p = subprocess.Popen([exe], stdin=subprocess.PIPE, stdout=subprocess.PIPE)
+        self.dir = tempfile.mkdtemp(prefix="stream_host_check_")   # per run: a shared /tmp may hold another user's build
+        exe = os.path.join(self.dir, "stream_host_check")
+        try:
+            subprocess.check_call(["g++", "-O1", "-std=c++17", "-I/usr/local/cuda/include", "-o", exe, os.path.join(ROOT, "tools", "stream_host_check.cpp")], stderr=subprocess.DEVNULL)
+            self.p = subprocess.Popen([exe], stdin=subprocess.PIPE, stdout=subprocess.PIPE)
+        except BaseException:
+            shutil.rmtree(self.dir, ignore_errors=True)
+            raise
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.p.kill(); self.p.wait(); self.p.stdin.close(); self.p.stdout.close()
+        shutil.rmtree(self.dir, ignore_errors=True)
 
     def open(self, kind, model, response_id=b"", created=0):
         self.p.stdin.write(("open %d %s %s %d\n" % (KIND[kind], model.decode() or "-", response_id.decode() or "-", created)).encode())
@@ -39,8 +55,12 @@ class Host:
 
 
 def main():
+    with Host() as H:
+        check(H)
+
+
+def check(H):
     T = load("test_messages_openai_response_gpu")
-    H = Host()
     # goldens under four chunkings
     for c in T.GOLD:
         req_model = json.loads(c["requestBody"])["model"].encode()
