@@ -7,6 +7,7 @@
 #include <sched.h>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
@@ -26,77 +27,145 @@
 
 using namespace aigw;
 
-struct aigw_cost_program { aigw::CelProgramHost h; };
+struct aigw_cost_program {
+  aigw::CelProgramHost h;
+  ~aigw_cost_program() { cudaFree(h.d_code); cudaFree(h.d_strings); }   // on the current device, like Scratch
+};
 
 // a failed call is reported once: its code is also taken off the thread's "last error", so that the launch check of a later call does not find it
 #define CK(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { ctx->err = std::string(#x) + ": " + cudaGetErrorString(_e); (void)cudaGetLastError(); return (int)_e; } } while (0)
+// Prologue of every int-returning C-ABI call that reaches the GPU: the context's device becomes current, checked like any other call
+// (a thread may have made another GPU current since the last call).  ENTER_ON also names the stream the call runs on: the caller's,
+// or the context's compute stream when the caller passes none.
+#define ENTER() CK(cudaSetDevice(ctx->device))
+#define ENTER_ON(stream) ENTER(); const cudaStream_t st = (stream) ? (cudaStream_t)(stream) : ctx->s_compute
+
+// An owning, grow-only scratch buffer of device memory or, Pinned, of mapped pinned host memory.  ensure(bytes) keeps it at least
+// `bytes` long: a shorter buffer is freed and reallocated with headroom (bytes + bytes/8 + 4096), so that a workload that creeps up
+// does not reallocate on every call; the contents are not kept.  The destructor frees it on the current device: aigw_destroy makes
+// the context's device current, and waits for its work, before the context's buffers go.
+template <class T, bool Pinned = false>
+struct Scratch {
+  T* p = nullptr;
+  size_t cap = 0;   // bytes
+  Scratch() = default;
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
+  ~Scratch() { release(); }
+  operator T*() const { return p; }
+  cudaError_t ensure(size_t bytes) {
+    if (cap >= bytes) return cudaSuccess;
+    release();
+    const size_t sz = bytes + bytes / 8 + 4096;
+    const cudaError_t e = Pinned ? cudaHostAlloc((void**)&p, sz, cudaHostAllocMapped) : cudaMalloc((void**)&p, sz);
+    if (e != cudaSuccess) { p = nullptr; return e; }
+    cap = sz;
+    return cudaSuccess;
+  }
+  void swap(Scratch& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
+
+ private:
+  void release() {
+    if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); }
+    p = nullptr; cap = 0;
+  }
+};
+template <class T> using PinnedScratch = Scratch<T, true>;
 
 static constexpr int kSlots = 3;
 static bool plain_json_text(const char* s) { for (; *s; s++) { unsigned char c = (unsigned char)*s; if (c < 0x20 || c > 0x7e || c == '"' || c == '\\') return false; } return true; }
 
 struct ChunkSlot {
-  uint8_t* d_in = nullptr; size_t in_cap = 0;
-  uint64_t* d_off = nullptr; uint32_t* d_len = nullptr; size_t doc_cap = 0;
-  uint32_t* d_map = nullptr; size_t map_cap = 0;   // size-class bucketing: documents of the chunk grouped by class
-  uint8_t* d_out = nullptr; size_t out_cap = 0;
-  aigw_doc_result* d_res = nullptr;
-  unsigned long long* d_used = nullptr;   // device bump counter
-  unsigned int* d_next = nullptr;         // device work counter
-  unsigned long long* h_used = nullptr;   // pinned mirror
+  Scratch<uint8_t> d_in;
+  Scratch<uint64_t> d_off; Scratch<uint32_t> d_len; Scratch<aigw_doc_result> d_res;
+  Scratch<uint32_t> d_map;   // size-class bucketing: documents of the chunk grouped by class
+  Scratch<uint8_t> d_out;
   cudaEvent_t ev_h2d, ev_k0, ev_k1, ev_ctr, ev_done;
 };
 
-struct aigw_bpe { uint2* d_table = nullptr; uint16_t* d_b2i = nullptr; uint32_t slots = 0; };
+struct aigw_bpe { Scratch<uint2> d_table; Scratch<uint16_t> d_b2i; uint32_t slots = 0; };
 
 struct aigw_ctx {
   int device = 0, sm_count = 0;
   cudaStream_t s_compute = nullptr, s_h2d = nullptr, s_d2h = nullptr;
   std::string err;
   // counters for the device API (ring so independent launches do not share a counter)
-  unsigned int* d_counters = nullptr; int counter_next = 0;
+  Scratch<unsigned int> d_counters; int counter_next = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   ChunkSlot slot[kSlots];
   // host-API output (pinned)
-  uint8_t* h_out = nullptr; size_t h_out_cap = 0;
-  aigw_doc_result* h_res = nullptr; size_t h_res_cap = 0;
+  PinnedScratch<uint8_t> h_out;
+  PinnedScratch<aigw_doc_result> h_res;
   long small_max = -1;   // aigw_chat_set_small_batch; -1: AIGW_SMALL_MAX or 512
   // BPE count (host form): device staging
-  uint8_t* d_bpe_text = nullptr; size_t bpe_text_cap = 0; uint64_t* d_bpe_off = nullptr; size_t bpe_off_cap = 0; uint32_t* d_bpe_len = nullptr; size_t bpe_len_cap = 0; uint32_t* d_bpe_cnt = nullptr; size_t bpe_cnt_cap = 0;
+  Scratch<uint8_t> d_bpe_text; Scratch<uint64_t> d_bpe_off; Scratch<uint32_t> d_bpe_len; Scratch<uint32_t> d_bpe_cnt;
   // large embeddings requests (aigw_embeddings_count_*): token workspace, text table, counts, host-form staging
-  uint32_t* d_emb_tok = nullptr; size_t emb_tok_cap = 0; uint64_t* d_emb_toff = nullptr; size_t emb_toff_cap = 0; uint32_t* d_emb_tlen = nullptr; size_t emb_tlen_cap = 0;
-  uint32_t* d_emb_cnt = nullptr; size_t emb_cnt_cap = 0; uint8_t* d_emb_body = nullptr; size_t emb_body_cap = 0; uint64_t* d_emb_off = nullptr; size_t emb_off_cap = 0;
-  uint32_t* d_emb_len = nullptr; size_t emb_len_cap = 0; aigw_emb_count_result* d_emb_res = nullptr; size_t emb_res_cap = 0;
-  uint8_t* h_small = nullptr; size_t h_small_cap = 0;   // small-batch path: tables + bodies, read by the kernel in place (mapped pinned)
+  Scratch<uint32_t> d_emb_tok; Scratch<uint64_t> d_emb_toff; Scratch<uint32_t> d_emb_tlen;
+  Scratch<uint32_t> d_emb_cnt; Scratch<uint8_t> d_emb_body; Scratch<uint64_t> d_emb_off;
+  Scratch<uint32_t> d_emb_len; Scratch<aigw_emb_count_result> d_emb_res;
+  PinnedScratch<uint8_t> h_small;   // small-batch path: tables + bodies, read by the kernel in place
   // chat workspace (intermediates of one sub-batch) + per-stage timing events
-  uint8_t* d_work = nullptr; size_t work_cap = 0;
-  unsigned long long* d_used_arr = nullptr; unsigned long long* h_used_arr = nullptr; size_t used_cap = 0;  // per-chunk bump counters
+  Scratch<uint8_t> d_work;
+  Scratch<unsigned long long> d_used_arr; PinnedScratch<unsigned long long> h_used_arr;  // per-chunk bump counters
   cudaEvent_t stage_ev[64]; float stage_ms[3] = {0, 0, 0}; int last_launches = 0;
   bool profile_stages = false;   // aigw_chat_set_profile: next device calls run the stages back to back on one stream and time them
   ChatAux aux{};                 // two extra streams: sub-batches of one call alternate between them
-  // sse host-API device buffers
-  uint8_t* d_sse_bytes = nullptr; size_t sse_bytes_cap = 0;
-  uint64_t* d_sse_coff = nullptr; size_t sse_coff_cap = 0;
-  uint32_t* d_sse_first = nullptr; size_t sse_first_cap = 0;
-  aigw_sse_result* d_sse_res = nullptr; size_t sse_res_cap = 0;
+  // device staging of the single-shot host calls (SSE usage, response usage, CEL costs, SHA-256); each call lays out its own
+  // tables in them, so their element types are only the common case
+  Scratch<uint8_t> stage_bytes;
+  Scratch<uint64_t> stage_off;
+  Scratch<uint32_t> stage_len;
+  Scratch<aigw_sse_result> stage_res;
   // bedrock stream workspace (records + counts) and host-API buffers
-  uint8_t* d_bs_work = nullptr; size_t bs_work_cap = 0;
-  uint64_t* d_bs_off[2] = {nullptr, nullptr}; size_t bs_off_cap[2] = {0, 0};
-  aigw_stream_result* h_sres = nullptr; size_t h_sres_cap = 0;
-  aigw_mut_result* h_mres = nullptr; size_t h_mres_cap = 0;
+  Scratch<uint8_t> d_bs_work;
+  Scratch<uint64_t> d_bs_off[2];
+  PinnedScratch<aigw_stream_result> h_sres;
+  PinnedScratch<aigw_mut_result> h_mres;
   std::vector<uint32_t> h_map;   // size-class bucketing scratch (host)
   // ---- stateful response streams (aigw_stream_*): device-resident slots + per-call staging
   struct StreamPool {
     std::mutex mu;
-    StreamSlot* d_slots = nullptr; uint32_t cap = 0;
+    Scratch<StreamSlot> d_slots; uint32_t cap = 0;   // cap: slots
     std::vector<uint32_t> free_list, carry, gen, stamp; std::vector<uint8_t> open; uint32_t call_no = 0;
-    uint8_t* h_in = nullptr; size_t h_in_cap = 0; uint8_t* d_in = nullptr; size_t d_in_cap = 0;
-    StreamStep* h_steps = nullptr; size_t h_steps_cap = 0; StreamStep* d_steps = nullptr; size_t d_steps_cap = 0;
-    aigw_chunk_result* d_res = nullptr; size_t d_res_cap = 0; aigw_chunk_result* h_res = nullptr; size_t h_res_cap = 0;
-    uint8_t* d_out = nullptr; size_t d_out_cap = 0; uint8_t* d_packed = nullptr; size_t d_packed_cap = 0; uint8_t* h_packed = nullptr; size_t h_packed_cap = 0;
-    unsigned long long* d_used = nullptr; unsigned long long* h_used = nullptr;
-    uint8_t* d_tmpl = nullptr; uint32_t* d_ids = nullptr; size_t d_ids_cap = 0; uint32_t* h_ids = nullptr; size_t h_ids_cap = 0;
+    PinnedScratch<uint8_t> h_in; Scratch<uint8_t> d_in;
+    PinnedScratch<StreamStep> h_steps; Scratch<StreamStep> d_steps;
+    Scratch<aigw_chunk_result> d_res; PinnedScratch<aigw_chunk_result> h_res;
+    Scratch<uint8_t> d_out; Scratch<uint8_t> d_packed; PinnedScratch<uint8_t> h_packed;
+    Scratch<unsigned long long> d_used; PinnedScratch<unsigned long long> h_used;
+    Scratch<uint8_t> d_tmpl; Scratch<uint32_t> d_ids; PinnedScratch<uint32_t> h_ids;
   } sp;
 };
+
+// k adjacent counters of the context's ring, zeroed on st
+static int take_counters(aigw_ctx* ctx, uint32_t k, cudaStream_t st, unsigned int** out) {
+  int at = ctx->counter_next & 255;
+  if (at + (int)k > 256) at = 0;
+  ctx->counter_next = at + (int)k;
+  *out = ctx->d_counters + at;
+  CK(cudaMemsetAsync(*out, 0, k * sizeof(unsigned int), st));
+  return 0;
+}
+
+// launch() on st; when kernel_ms is non-null, also wait for it and store its CUDA-event time there
+template <class F>
+static int timed(aigw_ctx* ctx, cudaStream_t st, float* kernel_ms, F&& launch) {
+  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
+  if (int rc = launch()) return rc;
+  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
+  return 0;
+}
+
+// Pipeline chunks of the host calls: chunk c is documents [cb[c], cb[c+1]).  A chunk holds at least one document and ends before
+// the first document i with end(i) - start(first document of the chunk) > budget.
+template <class S, class E>
+static std::vector<uint32_t> chunk_bounds(uint32_t n, uint64_t budget, S&& start, E&& end) {
+  std::vector<uint32_t> cb{0};
+  uint64_t s = start(0);
+  for (uint32_t i = 0; i < n; i++)
+    if (end(i) - s > budget && i > cb.back()) { cb.push_back(i); s = start(i); }
+  cb.push_back(n);
+  return cb;
+}
 
 // response bodies expand (escaped tool arguments, configuration text): plan them in a roomier size class
 static uint32_t resp_class_len(uint32_t max_len) { uint64_t m = (uint64_t)max_len * 4; if (m < 5120) m = 5120; if (m > 65536) m = max_len > 65536u ? max_len : 65536u; return (uint32_t)m; }
@@ -125,17 +194,6 @@ static void fill_params(ChatParams& P, const aigw_backend_cfg* cfg) {
     if (cfg->response_id) { size_t n = strlen(cfg->response_id); if (n > sizeof P.response_id) n = sizeof P.response_id; memcpy(P.response_id, cfg->response_id, n); P.rid_len = (uint16_t)n; }
   }
 }
-
-static int ensure(aigw_ctx* ctx, void** p, size_t* cap, size_t want, bool host) {
-  if (*cap >= want) return 0;
-  if (*p) { if (host) cudaFreeHost(*p); else cudaFree(*p); *p = nullptr; *cap = 0; }
-  size_t sz = want + want / 8 + 4096;
-  cudaError_t e = host ? cudaHostAlloc(p, sz, cudaHostAllocMapped) : cudaMalloc(p, sz);
-  if (e != cudaSuccess) { ctx->err = std::string(host ? "cudaHostAlloc" : "cudaMalloc") + ": " + cudaGetErrorString(e); return (int)e; }
-  *cap = sz;
-  return 0;
-}
-#define ENSURE(p, cap, want, host) do { int _r = ensure(ctx, (void**)&(p), &(cap), (want), (host)); if (_r) return _r; } while (0)
 
 namespace aigw {
 int ctx_device(const aigw_ctx* ctx) { return ctx->device; }
@@ -191,13 +249,12 @@ int aigw_init(int device, aigw_ctx** out) {
   for (int k = 0; k < kChatStreams; k++) { INIT_CK(cudaStreamCreateWithFlags(&ctx->aux.s[k], cudaStreamNonBlocking)); INIT_CK(cudaEventCreateWithFlags(&ctx->aux.join[k], cudaEventDisableTiming)); }
   INIT_CK(cudaEventCreateWithFlags(&ctx->aux.fork, cudaEventDisableTiming));
   for (int k = 0; k < kChatRing; k++) { INIT_CK(cudaEventCreateWithFlags(&ctx->aux.idx_done[k], cudaEventDisableTiming)); INIT_CK(cudaEventCreateWithFlags(&ctx->aux.walk_done[k], cudaEventDisableTiming)); INIT_CK(cudaEventCreateWithFlags(&ctx->aux.emit_done[k], cudaEventDisableTiming)); }
-  INIT_CK(cudaMalloc(&ctx->d_counters, 256 * sizeof(unsigned int)));
+  INIT_CK(ctx->d_counters.ensure(256 * sizeof(unsigned int)));
   INIT_CK(cudaEventCreate(&ctx->ev0)); INIT_CK(cudaEventCreate(&ctx->ev1));
   for (auto& e2 : ctx->stage_ev) INIT_CK(cudaEventCreate(&e2));
   for (auto& s : ctx->slot) {
     INIT_CK(cudaEventCreateWithFlags(&s.ev_h2d, cudaEventDisableTiming)); INIT_CK(cudaEventCreate(&s.ev_k0)); INIT_CK(cudaEventCreate(&s.ev_k1));
     INIT_CK(cudaEventCreateWithFlags(&s.ev_ctr, cudaEventDisableTiming)); INIT_CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
-    INIT_CK(cudaMalloc(&s.d_used, 8)); INIT_CK(cudaMalloc(&s.d_next, 4)); INIT_CK(cudaHostAlloc(&s.h_used, 8, cudaHostAllocDefault));
   }
 #undef INIT_CK
   *out = ctx;
@@ -209,19 +266,11 @@ void aigw_destroy(aigw_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   for (auto& s : ctx->slot) {
-    cudaFree(s.d_in); cudaFree(s.d_off); cudaFree(s.d_len); cudaFree(s.d_out); cudaFree(s.d_res); cudaFree(s.d_used); cudaFree(s.d_next); cudaFreeHost(s.h_used);
     cudaEventDestroy(s.ev_h2d); cudaEventDestroy(s.ev_k0); cudaEventDestroy(s.ev_k1); cudaEventDestroy(s.ev_ctr); cudaEventDestroy(s.ev_done);
   }
-  cudaFreeHost(ctx->h_out); cudaFreeHost(ctx->h_res); cudaFreeHost(ctx->h_small); cudaFree(ctx->d_bpe_text); cudaFree(ctx->d_bpe_off); cudaFree(ctx->d_bpe_len); cudaFree(ctx->d_bpe_cnt); cudaFree(ctx->d_emb_tok); cudaFree(ctx->d_emb_toff); cudaFree(ctx->d_emb_tlen); cudaFree(ctx->d_emb_cnt); cudaFree(ctx->d_emb_body); cudaFree(ctx->d_emb_off); cudaFree(ctx->d_emb_len); cudaFree(ctx->d_emb_res); cudaFree(ctx->d_counters); cudaFree(ctx->d_work); cudaFree(ctx->d_used_arr); cudaFreeHost(ctx->h_used_arr);
   for (auto& e2 : ctx->stage_ev) cudaEventDestroy(e2);
-  cudaFree(ctx->d_sse_bytes); cudaFree(ctx->d_sse_coff); cudaFree(ctx->d_sse_first); cudaFree(ctx->d_sse_res); cudaFree(ctx->d_bs_work); cudaFree(ctx->d_bs_off[0]); cudaFree(ctx->d_bs_off[1]); cudaFreeHost(ctx->h_sres); cudaFreeHost(ctx->h_mres);
   cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1);
   cudaStreamDestroy(ctx->s_compute); cudaStreamDestroy(ctx->s_h2d); cudaStreamDestroy(ctx->s_d2h);
-  {
-    auto& sp = ctx->sp;
-    cudaFree(sp.d_slots); cudaFreeHost(sp.h_in); cudaFree(sp.d_in); cudaFreeHost(sp.h_steps); cudaFree(sp.d_steps); cudaFree(sp.d_res); cudaFreeHost(sp.h_res);
-    cudaFree(sp.d_out); cudaFree(sp.d_packed); cudaFreeHost(sp.h_packed); cudaFree(sp.d_used); cudaFreeHost(sp.h_used); cudaFree(sp.d_tmpl); cudaFree(sp.d_ids); cudaFreeHost(sp.h_ids);
-  }
   for (int k = 0; k < kChatStreams; k++) { if (ctx->aux.s[k]) cudaStreamDestroy(ctx->aux.s[k]); if (ctx->aux.join[k]) cudaEventDestroy(ctx->aux.join[k]); }
   if (ctx->aux.fork) cudaEventDestroy(ctx->aux.fork);
   for (int k = 0; k < kChatRing; k++) { if (ctx->aux.idx_done[k]) cudaEventDestroy(ctx->aux.idx_done[k]); if (ctx->aux.walk_done[k]) cudaEventDestroy(ctx->aux.walk_done[k]); if (ctx->aux.emit_done[k]) cudaEventDestroy(ctx->aux.emit_done[k]); }
@@ -262,17 +311,16 @@ void* aigw_host_alloc(aigw_ctx* ctx, size_t bytes) { void* p = nullptr; cudaSetD
 void aigw_host_free(aigw_ctx*, void* p) { cudaFreeHost(p); }
 void* aigw_device_alloc(aigw_ctx* ctx, size_t bytes) { void* p = nullptr; cudaSetDevice(ctx->device); if (cudaMalloc(&p, bytes) != cudaSuccess) { ctx->err = "cudaMalloc failed"; return nullptr; } return p; }
 void aigw_device_free(aigw_ctx* ctx, void* p) { cudaSetDevice(ctx->device); cudaFree(p); }
-int aigw_memcpy_h2d(aigw_ctx* ctx, void* dst, const void* src, size_t bytes) { CK(cudaSetDevice(ctx->device)); CK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); return 0; }
-int aigw_memcpy_d2h(aigw_ctx* ctx, void* dst, const void* src, size_t bytes) { CK(cudaSetDevice(ctx->device)); CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); return 0; }
-int aigw_memset_d(aigw_ctx* ctx, void* dst, int v, size_t bytes) { CK(cudaSetDevice(ctx->device)); CK(cudaMemset(dst, v, bytes)); return 0; }
-int aigw_sync(aigw_ctx* ctx) { CK(cudaSetDevice(ctx->device)); CK(cudaDeviceSynchronize()); return 0; }
+int aigw_memcpy_h2d(aigw_ctx* ctx, void* dst, const void* src, size_t bytes) { ENTER(); CK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); return 0; }
+int aigw_memcpy_d2h(aigw_ctx* ctx, void* dst, const void* src, size_t bytes) { ENTER(); CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); return 0; }
+int aigw_memset_d(aigw_ctx* ctx, void* dst, int v, size_t bytes) { ENTER(); CK(cudaMemset(dst, v, bytes)); return 0; }
+int aigw_sync(aigw_ctx* ctx) { ENTER(); CK(cudaDeviceSynchronize()); return 0; }
 
 static int chat_translate_device_impl(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
                                       const uint32_t* d_lens, const uint32_t* d_doc_map, uint32_t first, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
                                       aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
   if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
+  ENTER_ON(stream);
   ChatParams P;
   fill_params(P, cfg);
   P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.out = d_out; P.out_capacity = out_capacity;
@@ -285,17 +333,17 @@ static int chat_translate_device_impl(aigw_ctx* ctx, const aigw_backend_cfg* cfg
     size_t need = chat_work_bytes_for(ml, n);
     const size_t cap = (size_t)3 << 30, floor1 = chat_work_bytes(ml, 1024);
     if (need > cap) need = cap > floor1 ? cap : floor1;
-    ENSURE(ctx->d_work, ctx->work_cap, need, false);
+    CK(ctx->d_work.ensure(need));
   }
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_chat_translate(P, ml, ctx->device, ctx->sm_count, st, ctx->d_work, ctx->work_cap, &ctx->aux, &ctx->last_launches, stages ? ctx->stage_ev : nullptr, 64, first));
-  if (kernel_ms) {
-    CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1));
-    if (stages) {
-      ctx->stage_ms[0] = ctx->stage_ms[1] = ctx->stage_ms[2] = 0;
-      const int nsb = ctx->last_launches / 4;
-      for (int sb = 0; sb < nsb && 4 * sb + 3 < 64; sb++) for (int k = 0; k < 3; k++) { float ms = 0; cudaEventElapsedTime(&ms, ctx->stage_ev[4 * sb + k], ctx->stage_ev[4 * sb + k + 1]); ctx->stage_ms[k] += ms; }
-    }
+  if (int rc = timed(ctx, st, kernel_ms, [&] {
+        CK(launch_chat_translate(P, ml, ctx->device, ctx->sm_count, st, ctx->d_work, ctx->d_work.cap, &ctx->aux, &ctx->last_launches, stages ? ctx->stage_ev : nullptr, 64, first));
+        return 0;
+      }))
+    return rc;
+  if (stages) {
+    ctx->stage_ms[0] = ctx->stage_ms[1] = ctx->stage_ms[2] = 0;
+    const int nsb = ctx->last_launches / 4;
+    for (int sb = 0; sb < nsb && 4 * sb + 3 < 64; sb++) for (int k = 0; k < 3; k++) { float ms = 0; cudaEventElapsedTime(&ms, ctx->stage_ev[4 * sb + k], ctx->stage_ev[4 * sb + k + 1]); ctx->stage_ms[k] += ms; }
   }
   return 0;
 }
@@ -329,10 +377,10 @@ static int chat_small_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uin
   uint64_t in_bytes = 0, out_bytes = 0;
   for (uint32_t i = 0; i < n; i++) { in_bytes += (((uint64_t)lens[i] + 15u) & ~15ull) + 16; out_bytes += ((uint64_t)lens[i] * 3 + 1024 + 15) & ~15ull; }
   const size_t tab = (((size_t)n + 1) * 16 + (size_t)n * 4 + 63) & ~(size_t)63;
-  ENSURE(ctx->h_small, ctx->h_small_cap, tab + in_bytes + 64, true);
-  ENSURE(ctx->h_out, ctx->h_out_cap, out_bytes + 64, true);
-  ENSURE(ctx->h_res, ctx->h_res_cap, (size_t)n * sizeof(aigw_doc_result), true);
-  uint64_t* h_off = (uint64_t*)ctx->h_small; uint64_t* h_slot = h_off + n + 1; uint32_t* h_len = (uint32_t*)(h_slot + n + 1);
+  CK(ctx->h_small.ensure(tab + in_bytes + 64));
+  CK(ctx->h_out.ensure(out_bytes + 64));
+  CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result)));
+  uint64_t* h_off = (uint64_t*)ctx->h_small.p; uint64_t* h_slot = h_off + n + 1; uint32_t* h_len = (uint32_t*)(h_slot + n + 1);
   uint8_t* h_in = ctx->h_small + tab;
   uint64_t o = 0, so = 0;
   for (uint32_t i = 0; i < n; i++) {
@@ -374,7 +422,7 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   // AIGW_HOST_ZEROCOPY=1 restores the round-1 variant (emit stores straight into mapped host memory) for A/B runs.
   memset(out, 0, sizeof *out);
   if (n == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
+  ENTER();
   {
     static const long env_small_max = getenv("AIGW_SMALL_MAX") ? atol(getenv("AIGW_SMALL_MAX")) : 512;   // 0 disables the fused small-batch path
     if ((long)n <= (ctx->small_max >= 0 ? ctx->small_max : env_small_max)) {
@@ -385,18 +433,9 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   }
   static const bool zero_copy = getenv("AIGW_HOST_ZEROCOPY") != nullptr;
   static const uint64_t kChunkBytes = (uint64_t)(getenv("AIGW_CHUNK_MB") ? atol(getenv("AIGW_CHUNK_MB")) : 256) << 20;   // pipeline granularity (fill / drain cost vs per-chunk launches)
-  std::vector<uint32_t> cb;  // chunk begin doc index
-  cb.push_back(0);
+  const std::vector<uint32_t> cb = chunk_bounds(n, kChunkBytes, [&](uint32_t i) { return offsets[i]; }, [&](uint32_t i) { return offsets[i] + (((uint64_t)lens[i] + 15u) & ~15ull); });
   uint32_t max_len = 0;
-  {
-    uint64_t start = offsets[0];
-    for (uint32_t i = 0; i < n; i++) {
-      const uint64_t end = offsets[i] + (((uint64_t)lens[i] + 15u) & ~15ull);
-      if (end - start > kChunkBytes && i > cb.back()) { cb.push_back(i); start = offsets[i]; }
-      if (lens[i] > max_len) max_len = lens[i];
-    }
-    cb.push_back(n);
-  }
+  for (uint32_t i = 0; i < n; i++) if (lens[i] > max_len) max_len = lens[i];
   const int nch = (int)cb.size() - 1;
   uint64_t max_in = 0, max_out = 0; uint32_t max_docs = 0;
   std::vector<uint64_t> in_bytes(nch), out_cap(nch), out_base(nch);
@@ -412,14 +451,9 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   const int nslots = nch < kSlots ? nch : kSlots;
   for (int s = 0; s < nslots; s++) {
     ChunkSlot& S = ctx->slot[s];
-    ENSURE(S.d_in, S.in_cap, max_in + 64, false);
-    if (!zero_copy) { ENSURE(S.d_out, S.out_cap, max_out + 64, false); }
-    if (S.doc_cap < max_docs) {
-      cudaFree(S.d_off); cudaFree(S.d_len); cudaFree(S.d_res); S.doc_cap = 0;
-      const size_t dc = max_docs + max_docs / 8 + 16;
-      CK(cudaMalloc(&S.d_off, dc * 8)); CK(cudaMalloc(&S.d_len, dc * 4)); CK(cudaMalloc(&S.d_res, dc * sizeof(aigw_doc_result)));
-      S.doc_cap = dc;
-    }
+    CK(S.d_in.ensure(max_in + 64));
+    if (!zero_copy) CK(S.d_out.ensure(max_out + 64));
+    CK(S.d_off.ensure((size_t)max_docs * 8)); CK(S.d_len.ensure((size_t)max_docs * 4)); CK(S.d_res.ensure((size_t)max_docs * sizeof(aigw_doc_result)));
   }
   const bool resp_dir = cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK;
   if (resp_dir) max_len = resp_class_len(max_len);
@@ -431,16 +465,11 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     const size_t cap = (size_t)3 << 30;   // the launcher walks a class in sub-batches that fit the workspace
     const size_t floor1 = chat_work_bytes(max_len, 1024);
     if (need > cap) need = cap > floor1 ? cap : floor1;
-    ENSURE(ctx->d_work, ctx->work_cap, need, false);
+    CK(ctx->d_work.ensure(need));
   }
-  ENSURE(ctx->h_out, ctx->h_out_cap, total_out_cap, true);
-  ENSURE(ctx->h_res, ctx->h_res_cap, (size_t)n * sizeof(aigw_doc_result), true);
-  if ((size_t)nch > ctx->used_cap) {
-    cudaFree(ctx->d_used_arr); cudaFreeHost(ctx->h_used_arr); ctx->used_cap = 0;
-    const size_t cap = (size_t)nch + 64;
-    CK(cudaMalloc(&ctx->d_used_arr, cap * 8)); CK(cudaHostAlloc(&ctx->h_used_arr, cap * 8, cudaHostAllocDefault));
-    ctx->used_cap = cap;
-  }
+  CK(ctx->h_out.ensure(total_out_cap));
+  CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result)));
+  CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
   uint8_t* dev_out = nullptr; aigw_doc_result* dev_res = nullptr;  // device views of the pinned arenas (zero-copy variant)
   if (zero_copy) { CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0)); CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_res, 0)); }
 
@@ -484,7 +513,7 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
       ctx->h_map.resize(nd);
       uint32_t cur[6]; for (int k = 0; k < 6; k++) cur[k] = cls_start[k];
       for (uint32_t i = b; i < e; i++) ctx->h_map[cur[cls_of(lens[i])]++] = i;
-      ENSURE(S.d_map, S.map_cap, (size_t)nd * 4, false);
+      CK(S.d_map.ensure((size_t)nd * 4));
       CK(cudaMemcpyAsync(S.d_map, ctx->h_map.data(), (size_t)nd * 4, cudaMemcpyHostToDevice, ctx->s_h2d));   // pageable source: staged before the call returns
       h2d += (uint64_t)nd * 4;
     }
@@ -499,14 +528,14 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     // documents keep their global index: kernels address offsets/lens/results with doc0 + i (or doc_map[i])
     if (n_cls <= 1) {
       int nl = 0;
-      CK(launch_chat_translate_range(P, b, nd, kClsMax[top_cls], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->work_cap, &ctx->aux, &nl));
+      CK(launch_chat_translate_range(P, b, nd, kClsMax[top_cls], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &ctx->aux, &nl));
       out->gpu_launches += nl;
     } else {
       P.doc_map = S.d_map;
       for (int k = 0; k < 6; k++) {
         if (!cls_cnt[k]) continue;
         int nl = 0;
-        CK(launch_chat_translate_range(P, cls_start[k], cls_cnt[k], kClsMax[k], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->work_cap, &ctx->aux, &nl));
+        CK(launch_chat_translate_range(P, cls_start[k], cls_cnt[k], kClsMax[k], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &ctx->aux, &nl));
         out->gpu_launches += nl;
       }
     }
@@ -527,7 +556,7 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
 int aigw_bpe_load(aigw_ctx* ctx, const uint16_t* byte_to_id, const uint32_t* merges, uint32_t n_merges, aigw_bpe** out) {
   if (!ctx || !byte_to_id || (!merges && n_merges) || !out || n_merges >= 65535u) return -2;
   for (uint32_t r = 0; r < n_merges * 3; r++) if (merges[r] >= 65536u) return -2;
-  CK(cudaSetDevice(ctx->device));
+  ENTER();
   uint32_t slots = 1024; while (slots < n_merges * 2u) slots <<= 1;
   if (bpe_smem_bytes(slots) > 220u * 1024u) { ctx->err = "aigw_bpe_load: merge table does not fit shared memory"; return -2; }
   std::vector<uint2> tab(slots, make_uint2(0xffffffffu, 0xffffffffu));
@@ -540,41 +569,36 @@ int aigw_bpe_load(aigw_ctx* ctx, const uint16_t* byte_to_id, const uint32_t* mer
     if (dup) continue;   // the first rank of a pair wins (a well-formed merge list has no duplicates)
     tab[s] = make_uint2(key, (r << 16) | merges[3 * r + 2]);
   }
-  aigw_bpe* b = new aigw_bpe();
+  std::unique_ptr<aigw_bpe> b(new aigw_bpe());   // freed with its buffers unless it is handed out
   b->slots = slots;
-  if (cudaMalloc(&b->d_table, (size_t)slots * 8) != cudaSuccess || cudaMalloc(&b->d_b2i, 512) != cudaSuccess) { cudaFree(b->d_table); delete b; return (int)cudaErrorMemoryAllocation; }
+  CK(b->d_table.ensure((size_t)slots * 8)); CK(b->d_b2i.ensure(512));
   CK(cudaMemcpy(b->d_table, tab.data(), (size_t)slots * 8, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(b->d_b2i, byte_to_id, 512, cudaMemcpyHostToDevice));
-  *out = b;
+  *out = b.release();
   return 0;
 }
-void aigw_bpe_free(aigw_ctx* ctx, aigw_bpe* b) { if (!b) return; if (ctx) cudaSetDevice(ctx->device); cudaFree(b->d_table); cudaFree(b->d_b2i); delete b; }
+void aigw_bpe_free(aigw_ctx* ctx, aigw_bpe* b) { if (!b) return; if (ctx) cudaSetDevice(ctx->device); delete b; }
 
 int aigw_bpe_count_device(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t* d_text, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n, uint32_t* d_counts,
                           void* stream, float* kernel_ms) {
   if (!ctx || !bpe) return -2;
   if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
+  ENTER_ON(stream);
   BpeParams P; P.text = d_text; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.counts = d_counts; P.table = bpe->d_table; P.slots = bpe->slots; P.byte_to_id = bpe->d_b2i;
-  P.next = ctx->d_counters + (ctx->counter_next++ & 255);
-  CK(cudaMemsetAsync(P.next, 0, sizeof(unsigned int), st));
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_bpe_count(P, ctx->sm_count, st));
-  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
-  return 0;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_bpe_count(P, ctx->sm_count, st)); return 0; });
 }
 
 int aigw_bpe_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t* text, const uint64_t* offsets, const uint32_t* lens, uint32_t n, uint32_t* counts,
                         uint64_t* h2d_bytes, uint64_t* d2h_bytes, float* kernel_ms) {
   if (!ctx || !bpe) return -2;
   if (n == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
+  ENTER();
   uint64_t nbytes = 0; for (uint32_t i = 0; i < n; i++) { const uint64_t e = offsets[i] + lens[i]; if (e > nbytes) nbytes = e; }
-  ENSURE(ctx->d_bpe_text, ctx->bpe_text_cap, nbytes + 64, false);
-  ENSURE(ctx->d_bpe_off, ctx->bpe_off_cap, (size_t)n * 8, false);
-  ENSURE(ctx->d_bpe_len, ctx->bpe_len_cap, (size_t)n * 4, false);
-  ENSURE(ctx->d_bpe_cnt, ctx->bpe_cnt_cap, (size_t)n * 4, false);
+  CK(ctx->d_bpe_text.ensure(nbytes + 64));
+  CK(ctx->d_bpe_off.ensure((size_t)n * 8));
+  CK(ctx->d_bpe_len.ensure((size_t)n * 4));
+  CK(ctx->d_bpe_cnt.ensure((size_t)n * 4));
   cudaStream_t st = ctx->s_compute;
   CK(cudaMemcpyAsync(ctx->d_bpe_text, text, nbytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(ctx->d_bpe_off, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
@@ -595,8 +619,7 @@ int aigw_embeddings_count_device(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8
   if (!ctx || !bpe) return -2;
   if (kernel_ms) kernel_ms[0] = kernel_ms[1] = kernel_ms[2] = kernel_ms[3] = 0;
   if (n == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
+  ENTER_ON(stream);
   // every input costs at least three request bytes (two quotes and a comma); one row per four bytes covers inputs of two characters and up,
   // a request that would overflow the table is declined (AIGW_R_ARENA_FULL)
   const uint64_t text_cap64 = total_bytes / 4 + 1024;
@@ -604,14 +627,13 @@ int aigw_embeddings_count_device(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8
   const uint32_t text_cap = (uint32_t)text_cap64;
   const uint32_t tok_cap = max_len / 2 + 64;
   const int grid = emb_scan_grid(ctx->sm_count);
-  ENSURE(ctx->d_emb_tok, ctx->emb_tok_cap, (size_t)grid * tok_cap * 4, false);
-  ENSURE(ctx->d_emb_toff, ctx->emb_toff_cap, (size_t)text_cap * 8, false);
-  ENSURE(ctx->d_emb_tlen, ctx->emb_tlen_cap, (size_t)text_cap * 4, false);
-  ENSURE(ctx->d_emb_cnt, ctx->emb_cnt_cap, (size_t)text_cap * 4, false);
-  unsigned int* c0 = ctx->d_counters + (ctx->counter_next++ & 255);
-  unsigned int* c1 = ctx->d_counters + (ctx->counter_next++ & 255);
-  unsigned int* c2 = ctx->d_counters + (ctx->counter_next++ & 255);
-  CK(cudaMemsetAsync(c0, 0, sizeof(unsigned int), st)); CK(cudaMemsetAsync(c1, 0, sizeof(unsigned int), st)); CK(cudaMemsetAsync(c2, 0, sizeof(unsigned int), st));
+  CK(ctx->d_emb_tok.ensure((size_t)grid * tok_cap * 4));
+  CK(ctx->d_emb_toff.ensure((size_t)text_cap * 8));
+  CK(ctx->d_emb_tlen.ensure((size_t)text_cap * 4));
+  CK(ctx->d_emb_cnt.ensure((size_t)text_cap * 4));
+  unsigned int* c0;
+  if (int rc = take_counters(ctx, 3, st, &c0)) return rc;
+  unsigned int* c1 = c0 + 1; unsigned int* c2 = c0 + 2;
   EmbScanParams E; E.bodies = d_bodies; E.offsets = d_offsets; E.lens = d_lens; E.n = n; E.results = d_results; E.tok_ws = ctx->d_emb_tok; E.tok_cap = tok_cap;
   E.text_off = ctx->d_emb_toff; E.text_len = ctx->d_emb_tlen; E.text_cap = text_cap; E.next = c0; E.text_used = c1;
   cudaEvent_t* ev = ctx->stage_ev;
@@ -641,13 +663,13 @@ int aigw_embeddings_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t
                                aigw_emb_count_result* results, uint64_t* h2d_bytes, uint64_t* d2h_bytes, float* kernel_ms) {
   if (!ctx || !bpe) return -2;
   if (n == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
+  ENTER();
   uint64_t nbytes = 0; uint32_t max_len = 0;
   for (uint32_t i = 0; i < n; i++) { const uint64_t e = offsets[i] + lens[i]; if (e > nbytes) nbytes = e; if (lens[i] > max_len) max_len = lens[i]; if (offsets[i] & 15u) { ctx->err = "aigw_embeddings_count_host: request starts must be 16-byte aligned"; return -2; } }
-  ENSURE(ctx->d_emb_body, ctx->emb_body_cap, nbytes + 64, false);
-  ENSURE(ctx->d_emb_off, ctx->emb_off_cap, (size_t)n * 8, false);
-  ENSURE(ctx->d_emb_len, ctx->emb_len_cap, (size_t)n * 4, false);
-  ENSURE(ctx->d_emb_res, ctx->emb_res_cap, (size_t)n * sizeof(aigw_emb_count_result), false);
+  CK(ctx->d_emb_body.ensure(nbytes + 64));
+  CK(ctx->d_emb_off.ensure((size_t)n * 8));
+  CK(ctx->d_emb_len.ensure((size_t)n * 4));
+  CK(ctx->d_emb_res.ensure((size_t)n * sizeof(aigw_emb_count_result)));
   cudaStream_t st = ctx->s_compute;
   CK(cudaMemcpyAsync(ctx->d_emb_body, bodies, nbytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(ctx->d_emb_off, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
@@ -664,36 +686,31 @@ int aigw_embeddings_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t
 int aigw_sse_usage_device(aigw_ctx* ctx, const uint8_t* d_bytes, const uint64_t* d_chunk_off, const uint32_t* d_chunk_first,
                           uint32_t n_streams, aigw_sse_result* d_results, void* stream, float* kernel_ms) {
   if (n_streams == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
+  ENTER_ON(stream);
   SseParams P; P.bytes = d_bytes; P.chunk_off = d_chunk_off; P.chunk_first = d_chunk_first; P.n_streams = n_streams; P.results = d_results;
-  P.next = ctx->d_counters + (ctx->counter_next++ & 255);
-  CK(cudaMemsetAsync(P.next, 0, sizeof(unsigned int), st));
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_sse_usage(P, ctx->sm_count, st));
-  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
-  return 0;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_sse_usage(P, ctx->sm_count, st)); return 0; });
 }
 
 int aigw_sse_usage_host(aigw_ctx* ctx, const uint8_t* bytes, const uint64_t* chunk_off, const uint32_t* chunk_first,
                         uint32_t n_streams, uint32_t n_chunks, aigw_sse_result* results, uint64_t* h2d_bytes, uint64_t* d2h_bytes, float* kernel_ms) {
   if (n_streams == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER();
   const uint64_t nbytes = chunk_off[n_chunks];
-  ENSURE(ctx->d_sse_bytes, ctx->sse_bytes_cap, nbytes + 64, false);
-  ENSURE(ctx->d_sse_coff, ctx->sse_coff_cap, ((size_t)n_chunks + 1) * 8, false);
-  ENSURE(ctx->d_sse_first, ctx->sse_first_cap, ((size_t)n_streams + 1) * 4, false);
-  ENSURE(ctx->d_sse_res, ctx->sse_res_cap, (size_t)n_streams * sizeof(aigw_sse_result), false);
+  CK(ctx->stage_bytes.ensure(nbytes + 64));
+  CK(ctx->stage_off.ensure(((size_t)n_chunks + 1) * 8));
+  CK(ctx->stage_len.ensure(((size_t)n_streams + 1) * 4));
+  CK(ctx->stage_res.ensure((size_t)n_streams * sizeof(aigw_sse_result)));
   cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->d_sse_bytes, bytes, nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_sse_coff, chunk_off, ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_sse_first, chunk_first, ((size_t)n_streams + 1) * 4, cudaMemcpyHostToDevice, st));
-  SseParams P; P.bytes = ctx->d_sse_bytes; P.chunk_off = ctx->d_sse_coff; P.chunk_first = ctx->d_sse_first; P.n_streams = n_streams; P.results = ctx->d_sse_res;
-  P.next = ctx->d_counters + (ctx->counter_next++ & 255);
-  CK(cudaMemsetAsync(P.next, 0, sizeof(unsigned int), st));
+  CK(cudaMemcpyAsync(ctx->stage_bytes, bytes, nbytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->stage_off, chunk_off, ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->stage_len, chunk_first, ((size_t)n_streams + 1) * 4, cudaMemcpyHostToDevice, st));
+  SseParams P; P.bytes = ctx->stage_bytes; P.chunk_off = ctx->stage_off; P.chunk_first = ctx->stage_len; P.n_streams = n_streams; P.results = ctx->stage_res;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
   CK(cudaEventRecord(ctx->ev0, st));
   CK(launch_sse_usage(P, ctx->sm_count, st));
   CK(cudaEventRecord(ctx->ev1, st));
-  CK(cudaMemcpyAsync(results, ctx->d_sse_res, (size_t)n_streams * sizeof(aigw_sse_result), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(results, ctx->stage_res, (size_t)n_streams * sizeof(aigw_sse_result), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1));
   if (h2d_bytes) *h2d_bytes = nbytes + ((uint64_t)n_chunks + 1) * 8 + ((uint64_t)n_streams + 1) * 4;
@@ -708,10 +725,10 @@ static int stream_pool_grow(aigw_ctx* ctx, uint32_t want) {
   uint32_t ncap = sp.cap ? sp.cap : 1024u;
   while (ncap < want) ncap *= 2;
   if (ncap > (1u << 22)) { ctx->err = "too many open streams"; return -3; }
-  StreamSlot* nd = nullptr;
-  CK(cudaMalloc(&nd, (size_t)ncap * sizeof(StreamSlot)));
-  if (sp.d_slots) { CK(cudaMemcpyAsync(nd, sp.d_slots, (size_t)sp.cap * sizeof(StreamSlot), cudaMemcpyDeviceToDevice, ctx->s_compute)); CK(cudaStreamSynchronize(ctx->s_compute)); cudaFree(sp.d_slots); }
-  sp.d_slots = nd;
+  Scratch<StreamSlot> nd;   // copy, then swap: the old slots are freed with nd, and so is nd when the copy fails
+  CK(nd.ensure((size_t)ncap * sizeof(StreamSlot)));
+  if (sp.cap) { CK(cudaMemcpyAsync(nd, sp.d_slots, (size_t)sp.cap * sizeof(StreamSlot), cudaMemcpyDeviceToDevice, ctx->s_compute)); CK(cudaStreamSynchronize(ctx->s_compute)); }
+  sp.d_slots.swap(nd);
   sp.carry.resize(ncap, 0); sp.gen.resize(ncap, 0); sp.stamp.resize(ncap, 0); sp.open.resize(ncap, 0);
   for (uint32_t i = ncap; i-- > sp.cap;) sp.free_list.push_back(i);
   sp.cap = ncap;
@@ -727,7 +744,7 @@ static bool stream_handle_ok(aigw_ctx* ctx, uint64_t h, uint32_t& slot) {
 int aigw_stream_open_batch(aigw_ctx* ctx, const aigw_stream_cfg* cfg, uint32_t n, uint64_t* handles) {
   if (!cfg || (n && !handles)) return -2;
   if (n == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
+  ENTER();
   auto& sp = ctx->sp;
   std::lock_guard<std::mutex> lk(sp.mu);
   const char* model = cfg->request_model ? cfg->request_model : ""; const char* id = cfg->response_id ? cfg->response_id : "";
@@ -740,9 +757,9 @@ int aigw_stream_open_batch(aigw_ctx* ctx, const aigw_stream_cfg* cfg, uint32_t n
   t->kind = (uint32_t)cfg->kind; t->beg = t->end = 0; t->flags = 0; t->tool_index = cfg->kind == AIGW_STREAM_GCP_ANTHROPIC ? -1 : 0; t->active_index = -1;
   t->created = cfg->created; t->model_len = (uint32_t)strlen(model); memcpy(t->model, model, t->model_len);
   if (cfg->kind == AIGW_STREAM_AWS_BEDROCK) { t->id_len = (uint32_t)strlen(id); memcpy(t->id, id, t->id_len); t->flags |= SF_HAVE_CREATED; }
-  if (!sp.d_tmpl) CK(cudaMalloc(&sp.d_tmpl, kStreamHdrBytes));
-  ENSURE(sp.d_ids, sp.d_ids_cap, (size_t)n * 4, false);
-  ENSURE(sp.h_ids, sp.h_ids_cap, (size_t)n * 4, true);
+  CK(sp.d_tmpl.ensure(kStreamHdrBytes));
+  CK(sp.d_ids.ensure((size_t)n * 4));
+  CK(sp.h_ids.ensure((size_t)n * 4));
   for (uint32_t i = 0; i < n; i++) {
     const uint32_t slot = sp.free_list.back(); sp.free_list.pop_back();
     sp.open[slot] = 1; sp.gen[slot]++; sp.carry[slot] = 0;
@@ -775,12 +792,11 @@ static int stream_chunks_core(aigw_ctx* ctx, uint32_t n, GET&& get, aigw_chunk_r
   auto& sp = ctx->sp;
   if (arena) *arena = nullptr;
   if (n == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
   static const bool prof = getenv("AIGW_STREAM_PROF") != nullptr;
   auto now = [] { return std::chrono::steady_clock::now(); };
   auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
   const auto t0 = now();
-  ENSURE(sp.h_steps, sp.h_steps_cap, (size_t)n * sizeof(StreamStep), true);
+  CK(sp.h_steps.ensure((size_t)n * sizeof(StreamStep)));
   sp.call_no++;
   uint64_t in_bytes = 0, out_bytes = 0;
   for (uint32_t i = 0; i < n; i++) {
@@ -798,13 +814,13 @@ static int stream_chunks_core(aigw_ctx* ctx, uint32_t n, GET&& get, aigw_chunk_r
     s.out_cap = (uint32_t)(oc > 0x7fffffffull ? 0x7fffffffull : oc);
     s.out_off = out_bytes; out_bytes += ((uint64_t)s.out_cap + 15u) & ~15ull;
   }
-  if (!zc_base) { ENSURE(sp.h_in, sp.h_in_cap, in_bytes + 16, true); ENSURE(sp.d_in, sp.d_in_cap, in_bytes + 16, false); }
-  ENSURE(sp.d_steps, sp.d_steps_cap, (size_t)n * sizeof(StreamStep), false);
-  ENSURE(sp.d_res, sp.d_res_cap, (size_t)n * sizeof(aigw_chunk_result), false);
-  ENSURE(sp.h_res, sp.h_res_cap, (size_t)n * sizeof(aigw_chunk_result), true);
-  ENSURE(sp.d_out, sp.d_out_cap, out_bytes + 16, false);
-  ENSURE(sp.d_packed, sp.d_packed_cap, out_bytes + 16, false);
-  if (!sp.d_used) { CK(cudaMalloc(&sp.d_used, 8)); CK(cudaHostAlloc(&sp.h_used, 8, cudaHostAllocDefault)); }
+  if (!zc_base) { CK(sp.h_in.ensure(in_bytes + 16)); CK(sp.d_in.ensure(in_bytes + 16)); }
+  CK(sp.d_steps.ensure((size_t)n * sizeof(StreamStep)));
+  CK(sp.d_res.ensure((size_t)n * sizeof(aigw_chunk_result)));
+  CK(sp.h_res.ensure((size_t)n * sizeof(aigw_chunk_result)));
+  CK(sp.d_out.ensure(out_bytes + 16));
+  CK(sp.d_packed.ensure(out_bytes + 16));
+  CK(sp.d_used.ensure(8)); CK(sp.h_used.ensure(8));
   const auto t1 = now();
   if (!zc_base) host_parallel_for(n, [&](uint32_t b, uint32_t e) { for (uint32_t i = b; i < e; i++) { const StreamCallIn c = get(i); if (c.len) memcpy(sp.h_in + sp.h_steps[i].in_off, c.bytes, c.len); } });   // no caller pointer is retained
   const auto t2 = now();
@@ -812,7 +828,7 @@ static int stream_chunks_core(aigw_ctx* ctx, uint32_t n, GET&& get, aigw_chunk_r
   if (!zc_base) CK(cudaMemcpyAsync(sp.d_in, sp.h_in, in_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(sp.d_steps, sp.h_steps, (size_t)n * sizeof(StreamStep), cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(sp.d_used, 0, 8, st));
-  StreamParams P; P.slots = sp.d_slots; P.in = zc_base ? zc_dev : sp.d_in; P.out = sp.d_out; P.packed = sp.d_packed; P.packed_used = sp.d_used; P.packed_cap = sp.d_packed_cap; P.steps = sp.d_steps; P.results = sp.d_res; P.n = n;
+  StreamParams P; P.slots = sp.d_slots; P.in = zc_base ? zc_dev : sp.d_in; P.out = sp.d_out; P.packed = sp.d_packed; P.packed_used = sp.d_used; P.packed_cap = sp.d_packed.cap; P.steps = sp.d_steps; P.results = sp.d_res; P.n = n;
   CK(launch_stream_steps(P, st));
   // results: straight into the caller's array when it is pinned (one DMA), else through the pinned staging array
   cudaPointerAttributes ra; const bool res_pinned = cudaPointerGetAttributes(&ra, results) == cudaSuccess && ra.type == cudaMemoryTypeHost;
@@ -822,9 +838,9 @@ static int stream_chunks_core(aigw_ctx* ctx, uint32_t n, GET&& get, aigw_chunk_r
   CK(cudaMemcpyAsync(sp.h_used, sp.d_used, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const auto t3 = now();
-  const uint64_t used = *sp.h_used < sp.d_packed_cap ? *sp.h_used : sp.d_packed_cap;
+  const uint64_t used = *sp.h_used < sp.d_packed.cap ? *sp.h_used : sp.d_packed.cap;
   if (used) {
-    ENSURE(sp.h_packed, sp.h_packed_cap, used + 16, true);
+    CK(sp.h_packed.ensure(used + 16));
     CK(cudaMemcpyAsync(sp.h_packed, sp.d_packed, used, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
@@ -837,6 +853,7 @@ static int stream_chunks_core(aigw_ctx* ctx, uint32_t n, GET&& get, aigw_chunk_r
 }
 }  // extern "C++"
 int aigw_stream_chunks(aigw_ctx* ctx, const aigw_chunk_in* in, uint32_t n, aigw_chunk_result* results, const uint8_t** arena) {
+  ENTER();
   std::lock_guard<std::mutex> lk(ctx->sp.mu);
   return stream_chunks_core(ctx, n, [&](uint32_t i) { return StreamCallIn{in[i].handle, in[i].bytes, in[i].len, in[i].eos}; }, results, arena, nullptr, nullptr);
 }
@@ -844,6 +861,7 @@ int aigw_stream_chunks(aigw_ctx* ctx, const aigw_chunk_in* in, uint32_t n, aigw_
  * When `base` is mapped pinned memory (aigw_host_alloc) the kernels read the chunks in place: no staging copy, no H2D of the bytes. */
 int aigw_stream_chunks_soa(aigw_ctx* ctx, const uint64_t* handles, const uint8_t* base, const uint64_t* off, const uint32_t* len, const uint8_t* eos, uint32_t n,
                            aigw_chunk_result* results, const uint8_t** arena) {
+  ENTER();
   std::lock_guard<std::mutex> lk(ctx->sp.mu);
   const uint8_t* zc_dev = nullptr;
   {
@@ -855,6 +873,7 @@ int aigw_stream_chunks_soa(aigw_ctx* ctx, const uint64_t* handles, const uint8_t
   return stream_chunks_core(ctx, n, [&](uint32_t i) { return StreamCallIn{handles[i], base + off[i], len[i], eos ? (uint32_t)eos[i] : 0u}; }, results, arena, zc_dev ? base : nullptr, zc_dev);
 }
 int aigw_stream_chunk(aigw_ctx* ctx, uint64_t handle, const uint8_t* bytes, uint32_t len, int eos, uint8_t* out, uint32_t out_cap, aigw_chunk_result* res) {
+  ENTER();
   std::lock_guard<std::mutex> lk(ctx->sp.mu);
   aigw_chunk_in in; in.handle = handle; in.bytes = bytes; in.len = len; in.eos = eos ? 1u : 0u;
   const uint8_t* arena = nullptr;
@@ -880,33 +899,27 @@ int aigw_bedrock_stream_device(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg
                                void* stream, float* kernel_ms) {
   if (kernel_ms) *kernel_ms = 0;
   if (n_streams == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER_ON(stream);
   BedrockStreamParams P;
   if (int rc = fill_stream_params(ctx, P, cfg)) return rc;
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
-  ENSURE(ctx->d_bs_work, ctx->bs_work_cap, bedrock_work_bytes(total_bytes, n_streams), false);
+  CK(ctx->d_bs_work.ensure(bedrock_work_bytes(total_bytes, n_streams)));
   P.bytes = d_bytes; P.stream_off = d_stream_off; P.off_base = 0; P.out_bias = 0; P.n_streams = n_streams; P.out = d_out; P.out_capacity = out_capacity; P.results = d_results;
   P.out_used = (unsigned long long*)d_out_used;
   bedrock_work_layout(P, ctx->d_bs_work, n_streams);
-  ctx->counter_next = (ctx->counter_next + 1) & ~1;   // two adjacent counters
-  P.next = ctx->d_counters + (ctx->counter_next & 255); ctx->counter_next += 2;
+  if (int rc = take_counters(ctx, 2, st, &P.next)) return rc;
   CK(cudaMemsetAsync(d_out_used, 0, sizeof(uint64_t), st));
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_bedrock_stream(P, ctx->sm_count, st));
-  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
-  return 0;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_bedrock_stream(P, ctx->sm_count, st)); return 0; });
 }
 int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, const uint8_t* bytes, const uint64_t* stream_off, uint32_t n_streams,
                              uint64_t out_capacity_hint, aigw_stream_batch_out* out) {
   memset(out, 0, sizeof *out);
   if (n_streams == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER();
   BedrockStreamParams P0;
   if (int rc = fill_stream_params(ctx, P0, cfg)) return rc;
   // sub-batches of ~64 MiB of stream bytes
   constexpr uint64_t kChunk = 64ull << 20;
-  std::vector<uint32_t> cb; cb.push_back(0);
-  { uint64_t start = stream_off[0]; for (uint32_t i = 1; i < n_streams; i++) if (stream_off[i + 1] - start > kChunk) { cb.push_back(i); start = stream_off[i]; } cb.push_back(n_streams); }
+  const std::vector<uint32_t> cb = chunk_bounds(n_streams, kChunk, [&](uint32_t i) { return stream_off[i]; }, [&](uint32_t i) { return stream_off[i + 1]; });
   const int nch = (int)cb.size() - 1;
   const uint64_t total_in = stream_off[n_streams] - stream_off[0];
   const double ratio = out_capacity_hint ? (double)out_capacity_hint / (double)(total_in + 1) : 2.0;
@@ -920,18 +933,13 @@ int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, 
   }
   const int nslots = nch < 2 ? 1 : 2;
   for (int k = 0; k < nslots; k++) {
-    ENSURE(ctx->slot[k].d_in, ctx->slot[k].in_cap, max_in + 64, false);
-    ENSURE(ctx->d_bs_off[k], ctx->bs_off_cap[k], ((size_t)max_n + 1) * 8, false);
+    CK(ctx->slot[k].d_in.ensure(max_in + 64));
+    CK(ctx->d_bs_off[k].ensure(((size_t)max_n + 1) * 8));
   }
-  ENSURE(ctx->d_bs_work, ctx->bs_work_cap, bedrock_work_bytes(max_in, max_n), false);
-  ENSURE(ctx->h_out, ctx->h_out_cap, total_cap, true);
-  ENSURE(ctx->h_sres, ctx->h_sres_cap, (size_t)n_streams * sizeof(aigw_stream_result), true);
-  if ((size_t)nch > ctx->used_cap) {
-    cudaFree(ctx->d_used_arr); cudaFreeHost(ctx->h_used_arr); ctx->used_cap = 0;
-    const size_t cap = (size_t)nch + 64;
-    CK(cudaMalloc(&ctx->d_used_arr, cap * 8)); CK(cudaHostAlloc(&ctx->h_used_arr, cap * 8, cudaHostAllocDefault));
-    ctx->used_cap = cap;
-  }
+  CK(ctx->d_bs_work.ensure(bedrock_work_bytes(max_in, max_n)));
+  CK(ctx->h_out.ensure(total_cap));
+  CK(ctx->h_sres.ensure((size_t)n_streams * sizeof(aigw_stream_result)));
+  CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
   uint8_t* dev_out = nullptr; aigw_stream_result* dev_res = nullptr;
   CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0));
   CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_sres, 0));
@@ -954,8 +962,7 @@ int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, 
     P.out = dev_out + out_base[c]; P.out_capacity = out_cap[c]; P.out_bias = out_base[c];
     P.results = dev_res + b; P.out_used = ctx->d_used_arr + c;
     bedrock_work_layout(P, ctx->d_bs_work, nd);
-    ctx->counter_next = (ctx->counter_next + 1) & ~1;
-    P.next = ctx->d_counters + (ctx->counter_next & 255); ctx->counter_next += 2;
+    if (int rc = take_counters(ctx, 2, ctx->s_compute, &P.next)) return rc;
     CK(launch_bedrock_stream(P, ctx->sm_count, ctx->s_compute));
     CK(cudaEventRecord(S.ev_k1, ctx->s_compute));
     out->gpu_launches += 2;
@@ -1049,19 +1056,14 @@ int aigw_body_mutate_device(aigw_ctx* ctx, const aigw_body_mutation* m, const ui
                             uint32_t max_len, uint8_t* d_out, uint64_t out_capacity, aigw_mut_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
   if (kernel_ms) *kernel_ms = 0;
   if (n == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER_ON(stream);
   MutateParams P;
   if (int rc = fill_mutate_params(ctx, P, m)) return rc;
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
   P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.out = d_out; P.out_capacity = out_capacity; P.out_bias = 0; P.results = d_results;
   P.out_used = (unsigned long long*)d_out_used;
-  P.next = ctx->d_counters + (ctx->counter_next++ & 255);
-  CK(cudaMemsetAsync(P.next, 0, sizeof(unsigned int), st));
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
   CK(cudaMemsetAsync(d_out_used, 0, sizeof(uint64_t), st));
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_body_mutate(P, max_len ? max_len : 65536u, ctx->sm_count, st));
-  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
-  return 0;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_body_mutate(P, max_len ? max_len : 65536u, ctx->sm_count, st)); return 0; });
 }
 int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
                           aigw_mut_batch_out* out) {
@@ -1069,23 +1071,15 @@ int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint
   // kernel stores records and results straight into mapped pinned host memory, one synchronisation at the end.
   memset(out, 0, sizeof *out);
   if (n == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER();
   MutateParams P0;
   if (int rc = fill_mutate_params(ctx, P0, m)) return rc;
   uint64_t extra = 0;
   for (uint32_t k = 0; k < P0.n_keys; k++) extra += P0.keys[k].memb_len + 2;
   const uint64_t kChunkBytes = 256ull << 20;
-  std::vector<uint32_t> cb; cb.push_back(0);
+  const std::vector<uint32_t> cb = chunk_bounds(n, kChunkBytes, [&](uint32_t i) { return offsets[i]; }, [&](uint32_t i) { return offsets[i] + lens[i]; });
   uint32_t max_len = 0;
-  {
-    uint64_t start = offsets[0];
-    for (uint32_t i = 0; i < n; i++) {
-      const uint64_t end = offsets[i] + lens[i];
-      if (end - start > kChunkBytes && i > cb.back()) { cb.push_back(i); start = offsets[i]; }
-      if (lens[i] > max_len) max_len = lens[i];
-    }
-    cb.push_back(n);
-  }
+  for (uint32_t i = 0; i < n; i++) if (lens[i] > max_len) max_len = lens[i];
   const int nch = (int)cb.size() - 1;
   std::vector<uint64_t> in_bytes(nch), out_cap(nch), out_base(nch);
   uint64_t max_in = 0, total_cap = 0; uint32_t max_docs = 0;
@@ -1099,17 +1093,12 @@ int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint
   const int nslots = nch < 2 ? 1 : 2;
   for (int k = 0; k < nslots; k++) {
     ChunkSlot& S = ctx->slot[k];
-    ENSURE(S.d_in, S.in_cap, max_in + 64, false);
-    if (S.doc_cap < max_docs) { cudaFree(S.d_off); cudaFree(S.d_len); S.doc_cap = 0; const size_t dc = (size_t)max_docs + max_docs / 8 + 16; CK(cudaMalloc(&S.d_off, dc * 8)); CK(cudaMalloc(&S.d_len, dc * 4)); S.doc_cap = dc; }
+    CK(S.d_in.ensure(max_in + 64));
+    CK(S.d_off.ensure((size_t)max_docs * 8)); CK(S.d_len.ensure((size_t)max_docs * 4));
   }
-  ENSURE(ctx->h_out, ctx->h_out_cap, total_cap, true);
-  ENSURE(ctx->h_mres, ctx->h_mres_cap, (size_t)n * sizeof(aigw_mut_result), true);
-  if ((size_t)nch > ctx->used_cap) {
-    cudaFree(ctx->d_used_arr); cudaFreeHost(ctx->h_used_arr); ctx->used_cap = 0;
-    const size_t cap = (size_t)nch + 64;
-    CK(cudaMalloc(&ctx->d_used_arr, cap * 8)); CK(cudaHostAlloc(&ctx->h_used_arr, cap * 8, cudaHostAllocDefault));
-    ctx->used_cap = cap;
-  }
+  CK(ctx->h_out.ensure(total_cap));
+  CK(ctx->h_mres.ensure((size_t)n * sizeof(aigw_mut_result)));
+  CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
   uint8_t* dev_out = nullptr; aigw_mut_result* dev_res = nullptr;
   CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0));
   CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_mres, 0));
@@ -1130,8 +1119,7 @@ int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint
     P.bodies = S.d_in - offsets[b]; P.offsets = S.d_off; P.lens = S.d_len; P.n = nd;
     P.out = dev_out + out_base[c]; P.out_capacity = out_cap[c]; P.out_bias = out_base[c]; P.results = dev_res + b;
     P.out_used = ctx->d_used_arr + c;
-    P.next = ctx->d_counters + (ctx->counter_next++ & 255);
-    CK(cudaMemsetAsync(P.next, 0, sizeof(unsigned int), ctx->s_compute));
+    if (int rc = take_counters(ctx, 1, ctx->s_compute, &P.next)) return rc;
     CK(launch_body_mutate(P, max_len, ctx->sm_count, ctx->s_compute));
     CK(cudaEventRecord(S.ev_k1, ctx->s_compute));
     out->gpu_launches += 1;
@@ -1150,12 +1138,8 @@ int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint
 static int sha_common(aigw_ctx* ctx, const uint8_t* d_bytes, const uint64_t* d_off, const uint32_t* d_len, const aigw_doc_result* d_res, uint32_t n, uint8_t* d_dig, void* stream, float* kernel_ms) {
   if (kernel_ms) *kernel_ms = 0;
   if (n == 0) return 0;
-  cudaSetDevice(ctx->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_sha256(d_bytes, d_off, d_len, d_res, n, d_dig, st));
-  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
-  return 0;
+  ENTER_ON(stream);
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_sha256(d_bytes, d_off, d_len, d_res, n, d_dig, st)); return 0; });
 }
 int aigw_sha256_device(aigw_ctx* ctx, const uint8_t* d_bytes, const uint64_t* d_off, const uint32_t* d_len, uint32_t n, uint8_t* d_digests, void* stream, float* kernel_ms) {
   return sha_common(ctx, d_bytes, d_off, d_len, nullptr, n, d_digests, stream, kernel_ms);
@@ -1165,20 +1149,20 @@ int aigw_chat_body_sha256_device(aigw_ctx* ctx, const uint8_t* d_out, const aigw
 }
 int aigw_sha256_host(aigw_ctx* ctx, const uint8_t* bytes, const uint64_t* off, const uint32_t* len, uint32_t n, uint8_t* digests) {
   if (n == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER();
   uint64_t lo = ~0ull, hi = 0;
   for (uint32_t i = 0; i < n; i++) { if (off[i] < lo) lo = off[i]; if (off[i] + len[i] > hi) hi = off[i] + len[i]; }
   const uint64_t nbytes = hi - lo;
   ChunkSlot& S = ctx->slot[0];
-  ENSURE(S.d_in, S.in_cap, nbytes + 64, false);
-  if (S.doc_cap < n) { cudaFree(S.d_off); cudaFree(S.d_len); S.doc_cap = 0; const size_t dc = (size_t)n + n / 8 + 16; CK(cudaMalloc(&S.d_off, dc * 8)); CK(cudaMalloc(&S.d_len, dc * 4)); S.doc_cap = dc; }
-  ENSURE(ctx->d_sse_res, ctx->sse_res_cap, (size_t)n * 32, false);
+  CK(S.d_in.ensure(nbytes + 64));
+  CK(S.d_off.ensure((size_t)n * 8)); CK(S.d_len.ensure((size_t)n * 4));
+  CK(ctx->stage_res.ensure((size_t)n * 32));
   cudaStream_t st = ctx->s_compute;
   CK(cudaMemcpyAsync(S.d_in, bytes + lo, nbytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(S.d_off, off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(S.d_len, len, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  CK(launch_sha256(S.d_in - lo, S.d_off, S.d_len, nullptr, n, (uint8_t*)ctx->d_sse_res, st));
-  CK(cudaMemcpyAsync(digests, ctx->d_sse_res, (size_t)n * 32, cudaMemcpyDeviceToHost, st));
+  CK(launch_sha256(S.d_in - lo, S.d_off, S.d_len, nullptr, n, (uint8_t*)ctx->stage_res.p, st));
+  CK(cudaMemcpyAsync(digests, ctx->stage_res, (size_t)n * 32, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return 0;
 }
@@ -1186,19 +1170,19 @@ int aigw_sha256_host(aigw_ctx* ctx, const uint8_t* bytes, const uint64_t* off, c
 // ------------------------------------------------------------------ CEL cost expressions
 int aigw_cost_compile(aigw_ctx* ctx, const char* expr, aigw_cost_program** out) {
   *out = nullptr;
-  cudaSetDevice(ctx->device);
-  aigw_cost_program* p = new aigw_cost_program();
+  ENTER();
+  std::unique_ptr<aigw_cost_program> p(new aigw_cost_program());   // freed with its device copies unless it is handed out
   std::string err;
   const int rc = cel_compile(expr ? expr : "", p->h, err);
-  if (rc) { ctx->err = std::string(rc == 1 ? "CEL expression outside the compiled subset: " : "CEL expression rejected: ") + err; delete p; return rc == 1 ? -2 : -3; }
+  if (rc) { ctx->err = std::string(rc == 1 ? "CEL expression outside the compiled subset: " : "CEL expression rejected: ") + err; return rc == 1 ? -2 : -3; }
   std::vector<CelInstr> padded(p->h.code); padded.resize(kCelMaxInstr, CelInstr{});
-  if (cudaMalloc(&p->h.d_code, sizeof(CelInstr) * kCelMaxInstr) != cudaSuccess || cudaMalloc(&p->h.d_strings, p->h.strings.size() + 16) != cudaSuccess) { ctx->err = "cudaMalloc"; delete p; return (int)cudaErrorMemoryAllocation; }
+  if (cudaMalloc(&p->h.d_code, sizeof(CelInstr) * kCelMaxInstr) != cudaSuccess || cudaMalloc(&p->h.d_strings, p->h.strings.size() + 16) != cudaSuccess) { ctx->err = "cudaMalloc"; return (int)cudaErrorMemoryAllocation; }
   CK(cudaMemcpy(p->h.d_code, padded.data(), sizeof(CelInstr) * kCelMaxInstr, cudaMemcpyHostToDevice));
   if (!p->h.strings.empty()) CK(cudaMemcpy(p->h.d_strings, p->h.strings.data(), p->h.strings.size(), cudaMemcpyHostToDevice));
-  *out = p;
+  *out = p.release();
   return 0;
 }
-void aigw_cost_program_free(aigw_ctx* ctx, aigw_cost_program* p) { if (!p) return; cudaSetDevice(ctx->device); cudaFree(p->h.d_code); cudaFree(p->h.d_strings); delete p; }
+void aigw_cost_program_free(aigw_ctx* ctx, aigw_cost_program* p) { if (!p) return; cudaSetDevice(ctx->device); delete p; }
 
 static int cel_fill(aigw_ctx* ctx, CelLaunch& L, aigw_cost_program* const* progs, uint32_t n_progs, const char* model, const char* backend, const char* route) {
   if (n_progs > (uint32_t)kCelMaxProgs) { ctx->err = "more than 8 CEL programs per call"; return -2; }
@@ -1223,36 +1207,36 @@ int aigw_usage_costs_cel_device(aigw_ctx* ctx, const aigw_sse_result* d_results,
                                 const uint8_t* d_model_bytes, const uint32_t* d_model_off, const uint32_t* d_model_len, const char* model, const char* backend,
                                 const char* route_name, uint64_t* d_costs, uint8_t* d_errs, void* stream) {
   if (n == 0 || n_progs == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER_ON(stream);
   CelLaunch L;
   if (int rc = cel_fill(ctx, L, progs, n_progs, model, backend, route_name)) return rc;
   L.results = d_results; L.n = n; L.model_bytes = d_model_bytes; L.model_off = d_model_off; L.model_len = d_model_len;
   L.costs = (unsigned long long*)d_costs; L.errs = d_errs;
-  CK(launch_cel(L, stream ? (cudaStream_t)stream : ctx->s_compute));
+  CK(launch_cel(L, st));
   return 0;
 }
 int aigw_usage_costs_cel_host(aigw_ctx* ctx, const aigw_sse_result* results, uint32_t n, aigw_cost_program* const* progs, uint32_t n_progs,
                               const uint8_t* model_bytes, uint64_t model_bytes_len, const uint32_t* model_off, const uint32_t* model_len, const char* model,
                               const char* backend, const char* route_name, uint64_t* costs, uint8_t* errs) {
   if (n == 0 || n_progs == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER();
   const size_t nres = (size_t)n * sizeof(aigw_sse_result), nout = (size_t)n * n_progs;
-  ENSURE(ctx->d_sse_res, ctx->sse_res_cap, nres, false);
-  ENSURE(ctx->d_sse_coff, ctx->sse_coff_cap, nout * 9 + 64, false);
-  ENSURE(ctx->d_sse_bytes, ctx->sse_bytes_cap, model_bytes_len + (size_t)n * 8 + 64, false);
+  CK(ctx->stage_res.ensure(nres));
+  CK(ctx->stage_off.ensure(nout * 9 + 64));   // costs, then error codes
+  CK(ctx->stage_bytes.ensure(model_bytes_len + (size_t)n * 8 + 64));
   cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->d_sse_res, results, nres, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->stage_res, results, nres, cudaMemcpyHostToDevice, st));
   uint32_t* d_off = nullptr; uint32_t* d_len = nullptr;
   if (model_off && model_len) {
-    d_off = (uint32_t*)ctx->d_sse_bytes; d_len = d_off + n;
+    d_off = (uint32_t*)ctx->stage_bytes.p; d_len = d_off + n;
     uint8_t* d_mb = (uint8_t*)(d_len + n);
     CK(cudaMemcpyAsync(d_off, model_off, (size_t)n * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_len, model_len, (size_t)n * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_mb, model_bytes, model_bytes_len, cudaMemcpyHostToDevice, st));
-    if (int rc = aigw_usage_costs_cel_device(ctx, ctx->d_sse_res, n, progs, n_progs, d_mb, d_off, d_len, model, backend, route_name, (uint64_t*)ctx->d_sse_coff, (uint8_t*)ctx->d_sse_coff + nout * 8, st)) return rc;
-  } else if (int rc = aigw_usage_costs_cel_device(ctx, ctx->d_sse_res, n, progs, n_progs, nullptr, nullptr, nullptr, model, backend, route_name, (uint64_t*)ctx->d_sse_coff, (uint8_t*)ctx->d_sse_coff + nout * 8, st)) return rc;
-  CK(cudaMemcpyAsync(costs, ctx->d_sse_coff, nout * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(errs, (uint8_t*)ctx->d_sse_coff + nout * 8, nout, cudaMemcpyDeviceToHost, st));
+    if (int rc = aigw_usage_costs_cel_device(ctx, ctx->stage_res, n, progs, n_progs, d_mb, d_off, d_len, model, backend, route_name, ctx->stage_off, (uint8_t*)ctx->stage_off.p + nout * 8, st)) return rc;
+  } else if (int rc = aigw_usage_costs_cel_device(ctx, ctx->stage_res, n, progs, n_progs, nullptr, nullptr, nullptr, model, backend, route_name, ctx->stage_off, (uint8_t*)ctx->stage_off.p + nout * 8, st)) return rc;
+  CK(cudaMemcpyAsync(costs, ctx->stage_off, nout * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(errs, (uint8_t*)ctx->stage_off.p + nout * 8, nout, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return 0;
 }
@@ -1260,11 +1244,8 @@ int aigw_usage_costs_cel_host(aigw_ctx* ctx, const aigw_sse_result* results, uin
 // ------------------------------------------------------------------ R1 + C2
 static int response_usage_device_impl(aigw_ctx* ctx, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
                                       aigw_sse_result* d_results, void* stream, float* kernel_ms, int embeddings) {
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
-  if (kernel_ms) CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_response_usage(d_bodies, d_offsets, d_lens, n, d_results, st, embeddings));
-  if (kernel_ms) { CK(cudaEventRecord(ctx->ev1, st)); CK(cudaEventSynchronize(ctx->ev1)); CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1)); }
-  return 0;
+  ENTER_ON(stream);
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_response_usage(d_bodies, d_offsets, d_lens, n, d_results, st, embeddings)); return 0; });
 }
 
 int aigw_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
@@ -1283,23 +1264,23 @@ int aigw_completions_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodie
 static int response_usage_host_impl(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
                                     const int32_t* cost_types, uint32_t n_costs, uint64_t* costs, int embeddings) {
   if (n == 0) return 0;
-  cudaSetDevice(ctx->device);
+  ENTER();
   const uint64_t nbytes = offsets[n - 1] + lens[n - 1] - offsets[0];
-  ENSURE(ctx->d_sse_bytes, ctx->sse_bytes_cap, nbytes + 64, false);
-  ENSURE(ctx->d_sse_coff, ctx->sse_coff_cap, ((size_t)n + 1) * 8 + (size_t)n_costs * 8 * n + 64, false);
-  ENSURE(ctx->d_sse_first, ctx->sse_first_cap, ((size_t)n + 1) * 4 + (size_t)n_costs * 4 + 64, false);
-  ENSURE(ctx->d_sse_res, ctx->sse_res_cap, (size_t)n * sizeof(aigw_sse_result), false);
+  CK(ctx->stage_bytes.ensure(nbytes + 64));
+  CK(ctx->stage_off.ensure(((size_t)n + 1) * 8 + (size_t)n_costs * 8 * n + 64));   // offsets, then costs
+  CK(ctx->stage_len.ensure(((size_t)n + 1) * 4 + (size_t)n_costs * 4 + 64));        // lengths, then cost types
+  CK(ctx->stage_res.ensure((size_t)n * sizeof(aigw_sse_result)));
   cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->d_sse_bytes, bodies + offsets[0], nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_sse_coff, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_sse_first, lens, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  CK(launch_response_usage(ctx->d_sse_bytes - offsets[0], ctx->d_sse_coff, ctx->d_sse_first, n, ctx->d_sse_res, st, embeddings));
-  CK(cudaMemcpyAsync(results, ctx->d_sse_res, (size_t)n * sizeof(aigw_sse_result), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(ctx->stage_bytes, bodies + offsets[0], nbytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->stage_off, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ctx->stage_len, lens, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  CK(launch_response_usage(ctx->stage_bytes - offsets[0], ctx->stage_off, ctx->stage_len, n, ctx->stage_res, st, embeddings));
+  CK(cudaMemcpyAsync(results, ctx->stage_res, (size_t)n * sizeof(aigw_sse_result), cudaMemcpyDeviceToHost, st));
   if (n_costs && costs) {
-    int32_t* d_types = (int32_t*)(ctx->d_sse_first + n + 1);
-    unsigned long long* d_costs = (unsigned long long*)(ctx->d_sse_coff + n + 1);
+    int32_t* d_types = (int32_t*)(ctx->stage_len + n + 1);
+    unsigned long long* d_costs = (unsigned long long*)(ctx->stage_off + n + 1);
     CK(cudaMemcpyAsync(d_types, cost_types, (size_t)n_costs * 4, cudaMemcpyHostToDevice, st));
-    CK(launch_usage_costs(ctx->d_sse_res, n, d_types, n_costs, d_costs, st));
+    CK(launch_usage_costs(ctx->stage_res, n, d_types, n_costs, d_costs, st));
     CK(cudaMemcpyAsync(costs, d_costs, (size_t)n * n_costs * 8, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
@@ -1319,7 +1300,7 @@ int aigw_completions_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, c
 }
 
 int aigw_usage_costs_device(aigw_ctx* ctx, const aigw_sse_result* d_results, uint32_t n, const int32_t* d_cost_types, uint32_t n_costs, uint64_t* d_costs, void* stream) {
-  cudaStream_t st = stream ? (cudaStream_t)stream : ctx->s_compute;
+  ENTER_ON(stream);
   CK(launch_usage_costs(d_results, n, d_cost_types, n_costs, (unsigned long long*)d_costs, st));
   return 0;
 }

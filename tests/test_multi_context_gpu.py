@@ -3,6 +3,7 @@ from two threads at once — the bench's --e2e-lanes mode and a gateway with sev
 second GPU, one context per device.  Every result is checked against the oracle."""
 import threading
 
+import numpy as np
 import pytest
 
 import _oracle as O
@@ -58,5 +59,34 @@ def test_one_context_per_device():
         for t in ts: t.start()
         for t in ts: t.join()
         assert not errors, errors[0]
+        _check_device_call_on_other_device(c0, c1)
     finally:
         c0.close(); c1.close()
+
+
+def _check_device_call_on_other_device(c0, c1):
+    """A device-buffer call of c1 made while this thread's current device is c0's still runs on c1's GPU."""
+    import aigw_b200 as A
+    n = 64
+    buf, coff, cfirst = W.sse_corpus(4, 0, n)
+    d = [c1.dalloc(a.nbytes) for a in (buf, coff, cfirst)] + [c1.dalloc(n * A.SseResult.itemsize)]
+    try:
+        for p, a in zip(d, (buf, coff, cfirst)):
+            c1.h2d(p, a)
+        c0.sync()   # makes c0's device current
+        c1.sse_usage_device(d[0], d[1], d[2], n, d[3])
+        res = np.zeros(n, dtype=A.SseResult)
+        c1.d2h(res, d[3])
+    finally:
+        for p in d:
+            c1.dfree(p)
+    raw = bytes(buf)
+    for s in range(n):
+        st = O.SSEStream(); acc = [-1] * 6
+        for c in range(int(cfirst[s]), int(cfirst[s + 1])):
+            u = st.feed(raw[int(coff[c]):int(coff[c + 1])]).as_tuple()
+            acc = [v if v >= 0 else a for a, v in zip(acc, u)]
+        r = res[s]; m = int(r["mask"])
+        got = [int(r["input"]) if m & 1 else -1, int(r["cached"]) if m & 8 else -1, int(r["cache_creation"]) if m & 16 else -1,
+               int(r["output"]) if m & 2 else -1, int(r["total"]) if m & 4 else -1, int(r["reasoning"]) if m & 32 else -1]
+        assert int(r["status"]) == 0 and got == acc, s

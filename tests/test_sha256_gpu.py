@@ -68,3 +68,22 @@ def test_translate_record_bodies(gw):
         body = bytes(out[o:o + int(r["body_len"])])
         assert r["status"] == 0 and bytes(dig[i]) == hashlib.sha256(body).digest()
     for p in (d_b, d_o, d_l, d_out, d_r, d_u, d_d): gw.dfree(p)
+
+
+def test_translate_host_after_larger_hash_host():
+    """the hash and translate host calls stage offsets and lengths in the same chunk slot: a translate call after a larger hash call
+    on a fresh context still gets a result table for its own batch"""
+    from aigw_b200 import capi
+    c = capi.Context(0)
+    try:
+        arena, offs, lens = W.chat_corpus(2, 0, 1200)
+        bodies = [bytes(arena[int(offs[i]):int(offs[i]) + int(lens[i])]) for i in range(1200)]
+        dig = c.sha256_host(arena, offs, lens)
+        assert all(bytes(dig[i]) == hashlib.sha256(bodies[i]).digest() for i in range(0, 1200, 50))
+        c.chat_set_small_batch(0)   # the throughput pipeline, which uses the chunk slots
+        got = c.chat_translate(c.cfg("aws-bedrock"), bodies[:1000])
+        for b, g in zip(bodies, got):
+            o = O.chat_translate("aws-bedrock", b)
+            assert g["status"] == 0 and o.status == O.OK and g["body"] == o.body and g["path"].decode() == o.path
+    finally:
+        c.close()
