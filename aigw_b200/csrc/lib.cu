@@ -748,7 +748,7 @@ int aigw_stream_open_batch(aigw_ctx* ctx, const aigw_stream_cfg* cfg, uint32_t n
   auto& sp = ctx->sp;
   std::lock_guard<std::mutex> lk(sp.mu);
   const char* model = cfg->request_model ? cfg->request_model : ""; const char* id = cfg->response_id ? cfg->response_id : "";
-  if (cfg->kind < AIGW_STREAM_OPENAI || cfg->kind > AIGW_STREAM_MESSAGES_AWS_ANTHROPIC || strlen(model) > 160 || strlen(id) > 160 || !plain_json_text(model) || !plain_json_text(id)) {
+  if (cfg->kind < AIGW_STREAM_OPENAI || cfg->kind > AIGW_STREAM_OPENAI_RESPONSES || strlen(model) > 160 || strlen(id) > 160 || !plain_json_text(model) || !plain_json_text(id)) {
     ctx->err = "stream cfg: unknown kind, or request_model / response_id need JSON escaping or exceed 160 bytes"; return -2;
   }
   if (sp.free_list.size() < n) { const int rc = stream_pool_grow(ctx, sp.cap + (uint32_t)(n - sp.free_list.size())); if (rc) return rc; }
@@ -1260,6 +1260,10 @@ int aigw_completions_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodie
                                            aigw_sse_result* d_results, void* stream, float* kernel_ms) {
   return response_usage_device_impl(ctx, d_bodies, d_offsets, d_lens, n, d_results, stream, kernel_ms, 2);
 }
+int aigw_responses_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
+                                           aigw_sse_result* d_results, void* stream, float* kernel_ms) {
+  return response_usage_device_impl(ctx, d_bodies, d_offsets, d_lens, n, d_results, stream, kernel_ms, 3);
+}
 
 static int response_usage_host_impl(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
                                     const int32_t* cost_types, uint32_t n_costs, uint64_t* costs, int embeddings) {
@@ -1297,6 +1301,10 @@ int aigw_embeddings_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, co
 int aigw_completions_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
                                          const int32_t* cost_types, uint32_t n_costs, uint64_t* costs) {
   return response_usage_host_impl(ctx, bodies, offsets, lens, n, results, cost_types, n_costs, costs, 2);
+}
+int aigw_responses_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
+                                         const int32_t* cost_types, uint32_t n_costs, uint64_t* costs) {
+  return response_usage_host_impl(ctx, bodies, offsets, lens, n, results, cost_types, n_costs, costs, 3);
 }
 
 int aigw_usage_costs_device(aigw_ctx* ctx, const aigw_sse_result* d_results, uint32_t n, const int32_t* d_cost_types, uint32_t n_costs, uint64_t* d_costs, void* stream) {

@@ -290,22 +290,30 @@ __global__ void __launch_bounds__(128) response_usage_kernel(const uint8_t* bodi
 
 // Buffered /v1/completions responses (openai_completions.go:98-150): json.Unmarshal of the whole body (no trailing bytes) into
 // openai.CompletionResponse; responseModel = resp.Model; every counter is set only when it is >= 0 — a negative or >= 2^31
-// counter is outside the integer captures' range and DECLINES.  The schema is read in place from device memory.
+// counter is outside the integer captures' range and DECLINES.
+// `responses`: buffered /v1/responses (openai_responses.go:117-142): json.NewDecoder(body).Decode(&openai.Response{}) (the first
+// value counts, trailing bytes are ignored); responseModel = cmp.Or(resp.Model, requestModel); a non-null usage sets all six
+// counters as uint32(int64), a null or absent one none.  The schemas are read in place from device memory.
 __device__ SchemaBlob g_cmpl_resp_schema;
-__global__ void __launch_bounds__(128) completions_response_kernel(const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results) {
+__device__ RspSchemaBlob g_rsp_resp_schema;
+__global__ void __launch_bounds__(128) completions_response_kernel(const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results, int responses) {
   const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= n) return;
   const uint8_t* p = bodies + offsets[d];
   Capture cp; cp.int_set = 0; cp.obj_seen = 0; cp.span_set = 0; cp.span_esc = 0; cp.weird = 0; cp.big = 0;
 #pragma unroll
   for (int k = 0; k < 8; k++) cp.ints[k] = 0;
-  const bool ok = walk(p, (int)lens[d], g_cmpl_resp_schema.nodes, g_cmpl_resp_schema.fields, g_cmpl_resp_schema.keys, N_ROOT, cp, /*allow_trailing=*/false);
+  const bool ok = responses ? walk<Capture, true>(p, (int)lens[d], g_rsp_resp_schema.nodes, g_rsp_resp_schema.fields, g_rsp_resp_schema.keys, X_ROOT, cp, /*allow_trailing=*/true)
+                            : walk(p, (int)lens[d], g_cmpl_resp_schema.nodes, g_cmpl_resp_schema.fields, g_cmpl_resp_schema.keys, N_ROOT, cp, /*allow_trailing=*/false);
   aigw_sse_result r; memset(&r, 0, sizeof r);
   if (cp.weird || (cp.span_esc & 1u)) r.status = AIGW_DECLINED;
   else if (!ok) r.status = AIGW_INTERNAL;  // "failed to unmarshal body"
   else {
     if (cp.obj_seen & (1u << C_OBJ_USAGE)) {
-      if (cp.big) r.status = AIGW_DECLINED;
+      if (responses) {
+        r.usage.input = cp.ints[C_PROMPT]; r.usage.output = cp.ints[C_COMPLETION]; r.usage.total = cp.ints[C_TOTAL];
+        r.usage.cached = cp.ints[C_CACHED]; r.usage.cache_creation = cp.ints[C_CACHE_CREATION]; r.usage.reasoning = cp.ints[C_REASONING]; r.usage.mask = 63u;
+      } else if (cp.big) r.status = AIGW_DECLINED;
       else {
         r.usage.input = cp.ints[C_PROMPT]; r.usage.output = cp.ints[C_COMPLETION]; r.usage.total = cp.ints[C_TOTAL]; r.usage.mask = 1u | 2u | 4u;
         if (cp.obj_seen & (1u << C_OBJ_PTD)) { r.usage.cached = cp.ints[C_CACHED]; r.usage.cache_creation = cp.ints[C_CACHE_CREATION]; r.usage.mask |= 8u | 16u; }
@@ -333,12 +341,13 @@ cudaError_t launch_response_usage(const uint8_t* bodies, const uint64_t* offsets
     const cudaError_t e0 = device_once(once, nullptr, [&](int*) {
       RespSchemaBlob b = build_resp_schema(); cudaError_t e = cudaMemcpyToSymbol(g_resp_schema, &b, sizeof b); if (e != cudaSuccess) return e;
       RespSchemaBlob b2 = build_emb_schema(); e = cudaMemcpyToSymbol(g_emb_schema, &b2, sizeof b2); if (e != cudaSuccess) return e;
-      SchemaBlob b3 = build_completion_schema(); return cudaMemcpyToSymbol(g_cmpl_resp_schema, &b3, sizeof b3);
+      SchemaBlob b3 = build_completion_schema(); e = cudaMemcpyToSymbol(g_cmpl_resp_schema, &b3, sizeof b3); if (e != cudaSuccess) return e;
+      RspSchemaBlob b4 = build_responses_schema(); return cudaMemcpyToSymbol(g_rsp_resp_schema, &b4, sizeof b4);
     });
     if (e0 != cudaSuccess) return e0;
   }
   if (n == 0) return cudaSuccess;
-  if (embeddings == 2) { completions_response_kernel<<<(n + 127) / 128, 128, 0, st>>>(bodies, offsets, lens, n, results); return cudaGetLastError(); }
+  if (embeddings >= 2) { completions_response_kernel<<<(n + 127) / 128, 128, 0, st>>>(bodies, offsets, lens, n, results, embeddings == 3); return cudaGetLastError(); }
   response_usage_kernel<<<(n + 127) / 128, 128, 0, st>>>(bodies, offsets, lens, n, results, embeddings);
   return cudaGetLastError();
 }

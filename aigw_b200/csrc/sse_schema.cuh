@@ -111,6 +111,107 @@ static inline SchemaBlob build_completion_schema() {
   return b;
 }
 
+// ------------------------------------------------------------------ schema: openai.Response (/v1/responses; walked by walk<CAP, true>)
+// Response :5845-6039, ResponseUsage :6663-6694, the output-item union :6147 (message :4013-4138 with the content and annotation
+// unions :4047-4266, function_call :4784, reasoning :4977), tools :2694 (function :2780), tool_choice :5654, instructions :6062,
+// text.format :2439-2522, reasoning :2525; the stream events response.created / response.completed :7729,7839.
+// Every tag the reference knows is listed: a tag this subset does not restate maps to X_DECL (DECLINE); any other tag fails.
+// The captured members come first in their object (the walker tracks repeats among the first 32 members only).
+enum XN : uint8_t { X_ANY = 0, X_STR, X_INT, X_FLOAT, X_BOOL, X_DECL, X_EVENT, X_ROOT, X_CREATED, X_PCREATED, X_F32, X_MODEL,
+                    X_ERROR, X_INCOMPLETE, X_INSTR, X_INSTR_ARR, X_STRMAP, X_ANYMAP, X_OUTPUT, X_ITEM, X_MSG, X_CONTENT, X_PARTS, X_PART,
+                    X_OTEXT, X_REFUSAL, X_ANNOTS, X_ANNOT, X_FCIT, X_UCIT, X_CCIT, X_FPATH, X_LPS, X_LP, X_INTS, X_TOPS, X_TOP,
+                    X_FCALL, X_RITEM, X_TEXTPARTS, X_TEXTPART, X_TC, X_TC_U, X_TC_FUNC, X_TOOLS, X_TOOL, X_FTOOL, X_CONV, X_PROMPT,
+                    X_REASONING, X_TEXT, X_FORMAT, X_FMT_TYPE, X_FMT_SCHEMA, X_USAGE, X_ITD, X_OTD,
+                    X_IN, X_OUT, X_TOTAL, X_CACHED, X_CREATION, X_REASONING_TOK, X_COUNT };
+enum : uint8_t { C_OBJ_RESPONSE = 3 };   // obj_seen bit: the event's `response` was a non-null object
+static const FieldDef kRspFields[] = {
+  {X_EVENT, "response", X_ROOT}, {X_EVENT, "type", X_STR}, {X_EVENT, "sequence_number", X_INT},
+  {X_ROOT, "model", X_MODEL}, {X_ROOT, "usage", X_USAGE}, {X_ROOT, "id", X_STR}, {X_ROOT, "created_at", X_CREATED}, {X_ROOT, "completed_at", X_PCREATED},
+  {X_ROOT, "error", X_ERROR}, {X_ROOT, "incomplete_details", X_INCOMPLETE}, {X_ROOT, "instructions", X_INSTR}, {X_ROOT, "metadata", X_STRMAP},
+  {X_ROOT, "object", X_STR}, {X_ROOT, "output", X_OUTPUT}, {X_ROOT, "parallel_tool_calls", X_BOOL}, {X_ROOT, "temperature", X_FLOAT},
+  {X_ROOT, "tool_choice", X_TC}, {X_ROOT, "tools", X_TOOLS}, {X_ROOT, "top_p", X_FLOAT}, {X_ROOT, "background", X_BOOL}, {X_ROOT, "conversation", X_CONV},
+  {X_ROOT, "max_output_tokens", X_INT}, {X_ROOT, "max_tool_calls", X_INT}, {X_ROOT, "previous_response_id", X_STR}, {X_ROOT, "prompt", X_PROMPT},
+  {X_ROOT, "prompt_cache_key", X_STR}, {X_ROOT, "prompt_cache_retention", X_STR}, {X_ROOT, "reasoning", X_REASONING}, {X_ROOT, "safety_identifier", X_STR},
+  {X_ROOT, "service_tier", X_STR}, {X_ROOT, "status", X_STR}, {X_ROOT, "text", X_TEXT}, {X_ROOT, "top_logprobs", X_INT}, {X_ROOT, "truncation", X_STR},
+  {X_ROOT, "user", X_STR}, {X_ROOT, "presence_penalty", X_F32}, {X_ROOT, "frequency_penalty", X_F32}, {X_ROOT, "store", X_BOOL},
+  {X_ERROR, "code", X_STR}, {X_ERROR, "message", X_STR},
+  {X_INCOMPLETE, "reason", X_STR},
+  {X_ITEM, "message", X_MSG}, {X_ITEM, "file_search_call", X_DECL}, {X_ITEM, "function_call", X_FCALL}, {X_ITEM, "function_call_output", X_DECL},
+  {X_ITEM, "web_search_call", X_DECL}, {X_ITEM, "computer_call", X_DECL}, {X_ITEM, "reasoning", X_RITEM}, {X_ITEM, "compaction", X_DECL},
+  {X_ITEM, "image_generation_call", X_DECL}, {X_ITEM, "code_interpreter_call", X_DECL}, {X_ITEM, "local_shell_call", X_DECL}, {X_ITEM, "shell_call", X_DECL},
+  {X_ITEM, "shell_call_output", X_DECL}, {X_ITEM, "apply_patch_call", X_DECL}, {X_ITEM, "apply_patch_call_output", X_DECL}, {X_ITEM, "mcp_call", X_DECL},
+  {X_ITEM, "mcp_list_tools", X_DECL}, {X_ITEM, "mcp_approval_request", X_DECL}, {X_ITEM, "custom_tool_call", X_DECL},
+  {X_MSG, "id", X_STR}, {X_MSG, "content", X_CONTENT}, {X_MSG, "status", X_STR}, {X_MSG, "role", X_STR}, {X_MSG, "type", X_STR},
+  {X_PART, "output_text", X_OTEXT}, {X_PART, "refusal", X_REFUSAL},
+  {X_OTEXT, "annotations", X_ANNOTS}, {X_OTEXT, "text", X_STR}, {X_OTEXT, "logprobs", X_LPS}, {X_OTEXT, "type", X_STR},
+  {X_REFUSAL, "refusal", X_STR}, {X_REFUSAL, "type", X_STR},
+  {X_ANNOT, "file_citation", X_FCIT}, {X_ANNOT, "url_citation", X_UCIT}, {X_ANNOT, "container_file_citation", X_CCIT}, {X_ANNOT, "file_path", X_FPATH},
+  {X_FCIT, "file_id", X_STR}, {X_FCIT, "filename", X_STR}, {X_FCIT, "index", X_INT}, {X_FCIT, "type", X_STR},
+  {X_UCIT, "end_index", X_INT}, {X_UCIT, "start_index", X_INT}, {X_UCIT, "title", X_STR}, {X_UCIT, "url", X_STR}, {X_UCIT, "type", X_STR},
+  {X_CCIT, "container_id", X_STR}, {X_CCIT, "end_index", X_INT}, {X_CCIT, "file_id", X_STR}, {X_CCIT, "filename", X_STR}, {X_CCIT, "start_index", X_INT}, {X_CCIT, "type", X_STR},
+  {X_FPATH, "file_id", X_STR}, {X_FPATH, "index", X_INT}, {X_FPATH, "type", X_STR},
+  {X_LP, "token", X_STR}, {X_LP, "bytes", X_INTS}, {X_LP, "logprob", X_FLOAT}, {X_LP, "top_logprobs", X_TOPS},
+  {X_TOP, "token", X_STR}, {X_TOP, "bytes", X_INTS}, {X_TOP, "logprob", X_FLOAT},
+  {X_FCALL, "arguments", X_STR}, {X_FCALL, "call_id", X_STR}, {X_FCALL, "name", X_STR}, {X_FCALL, "id", X_STR}, {X_FCALL, "status", X_STR}, {X_FCALL, "type", X_STR},
+  {X_RITEM, "id", X_STR}, {X_RITEM, "summary", X_TEXTPARTS}, {X_RITEM, "encrypted_content", X_STR}, {X_RITEM, "content", X_TEXTPARTS}, {X_RITEM, "status", X_STR}, {X_RITEM, "type", X_STR},
+  {X_TEXTPART, "text", X_STR}, {X_TEXTPART, "type", X_STR},
+  {X_TC_U, "allowed_tools", X_DECL}, {X_TC_U, "file_search", X_DECL}, {X_TC_U, "web_search_preview", X_DECL}, {X_TC_U, "computer_use_preview", X_DECL},
+  {X_TC_U, "web_search_preview_2025_03_11", X_DECL}, {X_TC_U, "image_generation", X_DECL}, {X_TC_U, "code_interpreter", X_DECL}, {X_TC_U, "function", X_TC_FUNC},
+  {X_TC_U, "mcp", X_DECL}, {X_TC_U, "custom", X_DECL}, {X_TC_U, "apply_patch", X_DECL}, {X_TC_U, "shell", X_DECL},
+  {X_TC_FUNC, "name", X_STR}, {X_TC_FUNC, "type", X_STR},
+  {X_TOOL, "function", X_FTOOL}, {X_TOOL, "file_search", X_DECL}, {X_TOOL, "computer_use_preview", X_DECL}, {X_TOOL, "web_search", X_DECL},
+  {X_TOOL, "web_search_2025_08_26", X_DECL}, {X_TOOL, "mcp", X_DECL}, {X_TOOL, "code_interpreter", X_DECL}, {X_TOOL, "image_generation", X_DECL},
+  {X_TOOL, "custom", X_DECL}, {X_TOOL, "local_shell", X_DECL}, {X_TOOL, "shell", X_DECL}, {X_TOOL, "web_search_preview", X_DECL},
+  {X_TOOL, "web_search_preview_2025_03_11", X_DECL}, {X_TOOL, "apply_patch", X_DECL},
+  {X_FTOOL, "strict", X_BOOL}, {X_FTOOL, "parameters", X_ANYMAP}, {X_FTOOL, "name", X_STR}, {X_FTOOL, "description", X_STR}, {X_FTOOL, "type", X_STR},
+  {X_CONV, "id", X_STR},
+  {X_PROMPT, "id", X_STR}, {X_PROMPT, "variables", X_DECL}, {X_PROMPT, "version", X_STR},
+  {X_REASONING, "effort", X_STR}, {X_REASONING, "generate_summary", X_STR}, {X_REASONING, "summary", X_STR},
+  {X_TEXT, "format", X_FORMAT}, {X_TEXT, "verbosity", X_STR},
+  {X_FORMAT, "text", X_FMT_TYPE}, {X_FORMAT, "json_schema", X_FMT_SCHEMA}, {X_FORMAT, "json_object", X_FMT_TYPE},
+  {X_FMT_TYPE, "type", X_STR},
+  {X_FMT_SCHEMA, "name", X_STR}, {X_FMT_SCHEMA, "schema", X_ANYMAP}, {X_FMT_SCHEMA, "strict", X_BOOL}, {X_FMT_SCHEMA, "description", X_STR}, {X_FMT_SCHEMA, "type", X_STR},
+  {X_USAGE, "input_tokens", X_IN}, {X_USAGE, "input_tokens_details", X_ITD}, {X_USAGE, "output_tokens", X_OUT}, {X_USAGE, "output_tokens_details", X_OTD},
+  {X_USAGE, "total_tokens", X_TOTAL},
+  {X_ITD, "cached_tokens", X_CACHED}, {X_ITD, "cache_creation_input_tokens", X_CREATION},
+  {X_OTD, "reasoning_tokens", X_REASONING_TOK},
+};
+static constexpr int kNumRspFields = sizeof(kRspFields) / sizeof(kRspFields[0]);
+struct alignas(16) RspSchemaBlob { Node nodes[X_COUNT]; Field fields[192]; char keys[2560]; };
+static_assert(kNumRspFields <= 192, "responses field table too small");
+
+static inline RspSchemaBlob build_responses_schema() {
+  RspSchemaBlob b; memset(&b, 0, sizeof b);
+  auto set = [&](int n, uint8_t kind, uint8_t cap = NOCAP, uint8_t elem = 0) { b.nodes[n].kind = kind; b.nodes[n].cap = cap; b.nodes[n].elem = elem; };
+  set(X_ANY, K_ANY); set(X_STR, K_STR); set(X_INT, K_INT); set(X_FLOAT, K_FLOAT); set(X_BOOL, K_BOOL); set(X_DECL, K_DECLINE);
+  set(X_EVENT, K_OBJ); set(X_ROOT, K_OBJ, C_OBJ_RESPONSE); set(X_CREATED, K_CREATED); set(X_PCREATED, K_PCREATED); set(X_F32, K_F32); set(X_MODEL, K_STR, C_SPAN_MODEL);
+  set(X_ERROR, K_OBJ); set(X_INCOMPLETE, K_OBJ);
+  set(X_INSTR, K_STROBJ, NOCAP, X_INSTR_ARR); set(X_INSTR_ARR, K_ARR, NOCAP, X_DECL);   // a string, null or []; input items are not restated
+  set(X_STRMAP, K_MAP, NOCAP, X_STR); set(X_ANYMAP, K_MAP, NOCAP, X_ANY);
+  set(X_OUTPUT, K_ARR, NOCAP, X_ITEM); set(X_ITEM, K_UNION); set(X_MSG, K_OBJ);
+  set(X_CONTENT, K_STRARR, NOCAP, X_PARTS); set(X_PARTS, K_ARR, NOCAP, X_PART); set(X_PART, K_UNION); set(X_OTEXT, K_OBJ); set(X_REFUSAL, K_OBJ);
+  set(X_ANNOTS, K_ARR, NOCAP, X_ANNOT); set(X_ANNOT, K_UNION); set(X_FCIT, K_OBJ); set(X_UCIT, K_OBJ); set(X_CCIT, K_OBJ); set(X_FPATH, K_OBJ);
+  set(X_LPS, K_ARR, NOCAP, X_LP); set(X_LP, K_OBJ); set(X_INTS, K_ARR, NOCAP, X_INT); set(X_TOPS, K_ARR, NOCAP, X_TOP); set(X_TOP, K_OBJ);
+  set(X_FCALL, K_OBJ); set(X_RITEM, K_OBJ); set(X_TEXTPARTS, K_ARR, NOCAP, X_TEXTPART); set(X_TEXTPART, K_OBJ);
+  set(X_TC, K_STROBJ, NOCAP, X_TC_U); set(X_TC_U, K_UNION); set(X_TC_FUNC, K_OBJ);   // "a string, else gjson type"
+  set(X_TOOLS, K_ARR, NOCAP, X_TOOL); set(X_TOOL, K_UNION); set(X_FTOOL, K_OBJ);
+  set(X_CONV, K_OBJ); set(X_PROMPT, K_OBJ); set(X_REASONING, K_OBJ); set(X_TEXT, K_OBJ); set(X_FORMAT, K_UNION); set(X_FMT_TYPE, K_OBJ); set(X_FMT_SCHEMA, K_OBJ);
+  set(X_USAGE, K_OBJ, C_OBJ_USAGE); set(X_ITD, K_OBJ); set(X_OTD, K_OBJ);
+  set(X_IN, K_INT, C_PROMPT); set(X_OUT, K_INT, C_COMPLETION); set(X_TOTAL, K_INT, C_TOTAL);
+  set(X_CACHED, K_INT, C_CACHED); set(X_CREATION, K_INT, C_CACHE_CREATION); set(X_REASONING_TOK, K_INT, C_REASONING);
+  int ko = 0;
+  for (int f = 0; f < kNumRspFields; f++) {
+    const FieldDef& d = kRspFields[f];
+    Node& o = b.nodes[d.owner];
+    if (o.nf == 0) o.f0 = (uint8_t)f;   // fields (and union tags) of one owner are contiguous in kRspFields
+    o.nf++;
+    int kl = (int)strlen(d.key);
+    b.fields[f].koff = (uint16_t)ko; b.fields[f].klen = (uint8_t)kl; b.fields[f].node = d.node;
+    memcpy(b.keys + ko, d.key, kl); ko += kl;
+  }
+  return b;
+}
+
 // ------------------------------------------------------------------ R1: non-stream ChatCompletionResponse usage
 // json.NewDecoder(body).Decode(&openai.ChatCompletionResponse{}) then usage / model
 // (internal/translator/openai_openai.go:146-174; struct internal/apischema/openai/openai.go:1269-1306,1365-1422).

@@ -14,6 +14,7 @@ namespace {
 __device__ SchemaBlob g_chunk_schema;        // openai.ChatCompletionResponseChunk
 __device__ SchemaBlob g_cmpl_schema;         // openai.CompletionResponse (legacy /v1/completions)
 __device__ RespSchemaBlob g_o2a_resp_schema; // openai.ChatCompletionResponse (buffered /v1/messages response of an OpenAI backend)
+__device__ RspSchemaBlob g_rsp_schema;       // openai.Response and its stream events (/v1/responses)
 __device__ BedrockSchema g_conv_schema;      // awsbedrock.ConverseStreamEvent
 __device__ uint32_t g_crc_tab[256];          // IEEE CRC-32
 
@@ -948,6 +949,55 @@ __device__ void step_anthropic_native(StreamSlot& S, const StreamStep& st, uint8
   if (ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k]; R.model_len = ml; }
 }
 
+// ------------------------------------------------------------------ S1 variant: /v1/responses, usage scan only
+// (openAIToOpenAITranslatorV1Responses.ResponseBody stream branch: handleStreamingResponse + extractUsageFromBufferEvent,
+//  internal/translator/openai_responses.go:102-114,146-192).  The reference keeps NO carry: every call splits only its own bytes into
+//  lines (a line cut across two calls is lost) and parses the last one even without a newline, so the step reads the call's bytes in
+//  place from the staged input and the slot holds only the stream's model.  A line counts when it starts with "data: " and its
+//  first top-level "type" is response.created (model) or response.completed (all six counters, cache creation 0, last one of the
+//  call wins); other events change nothing and are not validated.  A response.completed without usage DECLINES (the reference
+//  dereferences the nil *ResponseUsage).  It runs in its own kernel (stream_responses_kernel): the shared step kernel's code and frame
+//  stay as they were.
+__device__ void step_openai_responses(StreamSlot& S, const StreamStep& st, const uint8_t* b, uint8_t* out, aigw_chunk_result& R) {
+  const uint32_t n = st.len;
+  aigw_usage u; memset(&u, 0, sizeof u);
+  int status = 0;
+  for (uint32_t pos = 0; pos < n && !status;) {
+    uint32_t nl = pos; while (nl < n && b[nl] != '\n') nl++;
+    const uint8_t* line = b + pos; const uint32_t ll = nl - pos;
+    pos = nl + 1;
+    if (!prefix(line, ll, "data: ", 6)) continue;
+    const uint8_t* d = line + 6; const int dl = (int)ll - 6;
+    const int r0 = skipws(d, 0, dl);
+    if (r0 >= dl || d[r0] != '{') continue;   // empty data, [DONE], or no "type" to find
+    int ts = 0, tl = 0; const int r = union_tag(d, r0, dl, ts, tl);
+    if (r == -2) { status = AIGW_DECLINED; break; }
+    if (r <= 0) continue;
+    const bool created = EQ(d + ts, (uint32_t)tl, "response.created");
+    if (!created && !EQ(d + ts, (uint32_t)tl, "response.completed")) continue;
+    Capture cp; cap_reset(cp);
+    const bool ok = walk<Capture, true>(d, dl, g_rsp_schema.nodes, g_rsp_schema.fields, g_rsp_schema.keys, X_EVENT, cp);
+    if (cp.weird || (cp.span_esc & 1u)) { status = AIGW_DECLINED; break; }
+    if (!ok) continue;   // a decode error skips the line
+    if (created) {
+      if ((cp.span_set & 1u) && cp.span_len[0] > 0) {
+        if (cp.span_len[0] > sizeof S.rmodel) { status = AIGW_DECLINED; break; }
+        for (uint32_t k = 0; k < cp.span_len[0]; k++) S.rmodel[k] = (char)d[cp.span_off[0] + k];
+        S.rmodel_len = cp.span_len[0];
+      }
+    } else {
+      if (!(cp.obj_seen & (1u << C_OBJ_RESPONSE)) || !(cp.obj_seen & (1u << C_OBJ_USAGE))) { status = AIGW_DECLINED; break; }
+      u.input = cp.ints[C_PROMPT]; u.output = cp.ints[C_COMPLETION]; u.total = cp.ints[C_TOTAL];
+      u.cached = cp.ints[C_CACHED]; u.cache_creation = 0; u.reasoning = cp.ints[C_REASONING]; u.mask = 63u;
+    }
+  }
+  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = AIGW_R_UNSUPPORTED_FIELD; return; }
+  R.usage = u; R.body_kind = AIGW_BODY_UNCHANGED; R.out_len = 0;
+  // responseModel = cmp.Or(streamingResponseModel, requestModel)
+  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;
+  if (ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k]; R.model_len = ml; }
+}
+
 #include "stream_messages_openai.cuh"
 #include "stream_messages_aws_anthropic.cuh"
 
@@ -966,6 +1016,7 @@ __global__ void __launch_bounds__(128) stream_append_kernel(const __grid_constan
   const StreamStep st = P.steps[warp];
   StreamSlot& S = P.slots[st.slot];
   if (S.flags & SF_DEAD) return;
+  if (S.kind == AIGW_STREAM_OPENAI_RESPONSES) return;   // no carry: the step reads the call's bytes in place (beg = end = 0 stays)
   const uint32_t beg = S.beg, end = S.end, n = end - beg;
   if (lane == 0) S._r0 = n;   // carry length before this call (the Gemini step restates bufferedBody from it)
   if (beg) {   // move the carry to the front (reads of one batch complete before its writes; later batches read further right)
@@ -1016,6 +1067,21 @@ __global__ void __launch_bounds__(64) stream_step_kernel(const __grid_constant__
   P.results[i] = R;
 }
 
+// /v1/responses steps: the shared step kernel leaves them DECLINED (a kind it does not know); this kernel runs after it and writes
+// their results.  It reads the call's bytes in place: there is no carry.
+__global__ void __launch_bounds__(64) stream_responses_kernel(const __grid_constant__ StreamParams P) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n) return;
+  const StreamStep st = P.steps[i];
+  StreamSlot& S = P.slots[st.slot];
+  if (S.kind != AIGW_STREAM_OPENAI_RESPONSES) return;
+  aigw_chunk_result R; memset(&R, 0, sizeof R);
+  R.out_off = st.out_off;
+  if (S.flags & SF_DEAD) { R.status = (uint8_t)S.dead_status; R.reason = (uint8_t)S.dead_reason; }
+  else step_openai_responses(S, st, P.in + st.in_off, P.out + st.out_off, R);
+  P.results[i] = R;   // carry_len 0
+}
+
 __global__ void __launch_bounds__(128) stream_pack_kernel(const __grid_constant__ StreamParams P) {
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= P.n) return;
@@ -1046,6 +1112,7 @@ cudaError_t launch_stream_steps(const StreamParams& P, cudaStream_t st) {
       SchemaBlob a = build_schema(); cudaError_t e = cudaMemcpyToSymbol(g_chunk_schema, &a, sizeof a); if (e != cudaSuccess) return e;
       a = build_completion_schema(); e = cudaMemcpyToSymbol(g_cmpl_schema, &a, sizeof a); if (e != cudaSuccess) return e;
       { RespSchemaBlob r = build_resp_schema(); e = cudaMemcpyToSymbol(g_o2a_resp_schema, &r, sizeof r); if (e != cudaSuccess) return e; }
+      { RspSchemaBlob r = build_responses_schema(); e = cudaMemcpyToSymbol(g_rsp_schema, &r, sizeof r); if (e != cudaSuccess) return e; }
       BedrockSchema b = build_schema_bedrock(); e = cudaMemcpyToSymbol(g_conv_schema, &b, sizeof b); if (e != cudaSuccess) return e;
       AnSchema c = build_an_schema(); e = cudaMemcpyToSymbol(g_an_schema, &c, sizeof c); if (e != cudaSuccess) return e;
       uint32_t tab[256];
@@ -1057,6 +1124,7 @@ cudaError_t launch_stream_steps(const StreamParams& P, cudaStream_t st) {
   if (P.n == 0) return cudaSuccess;
   stream_append_kernel<<<(P.n * 32 + 127) / 128, 128, 0, st>>>(P);
   stream_step_kernel<<<(P.n + 63) / 64, 64, 0, st>>>(P);
+  stream_responses_kernel<<<(P.n + 63) / 64, 64, 0, st>>>(P);
   stream_pack_kernel<<<(P.n * 32 + 127) / 128, 128, 0, st>>>(P);
   return cudaGetLastError();
 }

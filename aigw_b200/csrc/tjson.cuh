@@ -12,7 +12,14 @@
 namespace aigw { namespace tj {
 
 enum Kind : uint8_t { K_ANY = 0, K_STR, K_INT, K_FLOAT, K_BOOL, K_OBJ, K_ARR, K_CREATED, K_B64, K_STROBJ /* string, or the object node in `elem` */,
-                      K_MAP /* map[string]T: an object with arbitrary keys whose values are all of node `elem` */ };
+                      K_MAP /* map[string]T: an object with arbitrary keys whose values are all of node `elem` */,
+                      // the kinds below are walked only by walk<CAP, true> (the Responses API schema); the other schemas compile without them
+                      K_UNION /* tagged union: an object whose first top-level "type" string picks the variant node from the tag table
+                                 fields[f0, f0+nf) (key = tag); null, a non-object, an unknown tag or a missing / non-string "type" fail */,
+                      K_STRARR /* a string, or the array node in `elem`; anything else, null included, fails */,
+                      K_DECLINE /* a member the schema knows but does not restate: any value sets `weird` */,
+                      K_PCREATED /* *JSONUNIXTime: null is nil, anything else as K_CREATED */,
+                      K_F32 /* float32: a number; an exponent or more than 38 integer digits (range not restated) sets `weird` */ };
 
 struct Field { uint16_t koff; uint8_t klen; uint8_t node; };  // key bytes at keys[koff..koff+klen)
 struct Node { uint8_t kind; uint8_t cap; uint8_t f0; uint8_t nf; uint8_t elem; };
@@ -138,8 +145,35 @@ __device__ inline int skip_any(const uint8_t* p, int i, int n) {
   }
 }
 
-// Typed walk of p[0..n).  Returns true when json.Unmarshal into the schema's root type would succeed.
-template <class CAP>
+// gjson.GetBytes(data, "type") on the object at p[i] == '{': the first top-level "type" member.  1: a string, its contents at
+// p[ts, ts+tl); 0: absent or not a string; -1: syntax error before it; -2: an escaped member name before it, or an escaped tag.
+__device__ inline int union_tag(const uint8_t* p, int i, int n, int& ts, int& tl) {
+  i++;
+  for (;;) {
+    while (i < n && ws(p[i])) i++;
+    if (i >= n) return -1;
+    if (p[i] == '}') return 0;
+    if (p[i] == ',') { i++; while (i < n && ws(p[i])) i++; }
+    if (i >= n || p[i] != '"') return -1;
+    bool e = false; const int j = scan_string(p, i, n, e); if (j < 0) return -1;
+    if (e) return -2;
+    const bool is_type = j - i == 6 && p[i + 1] == 't' && p[i + 2] == 'y' && p[i + 3] == 'p' && p[i + 4] == 'e';
+    i = j; while (i < n && ws(p[i])) i++;
+    if (i >= n || p[i] != ':') return -1;
+    i++; while (i < n && ws(p[i])) i++;
+    if (is_type) {
+      if (i >= n || p[i] != '"') return 0;
+      bool e2 = false; const int k = scan_string(p, i, n, e2); if (k < 0) return -1;
+      if (e2) return -2;
+      ts = i + 1; tl = k - i - 2; return 1;
+    }
+    i = skip_any(p, i, n); if (i < 0) return -1;
+  }
+}
+
+// Typed walk of p[0..n).  Returns true when json.Unmarshal into the schema's root type would succeed.  EXT: the schema uses the
+// kinds from K_UNION on.
+template <class CAP, bool EXT = false>
 __device__ inline bool walk(const uint8_t* p, int n, const Node* nodes, const Field* fields, const char* keys, int root, CAP& cap, bool allow_trailing = false) {
   const int MAXD = 12;
   uint8_t st_node[MAXD]; uint32_t st_seen[MAXD];
@@ -153,6 +187,29 @@ __device__ inline bool walk(const uint8_t* p, int n, const Node* nodes, const Fi
     Node nd = nodes[node];
     uint32_t c = p[i];
     if (nd.kind == K_STROBJ) { if (c == '"' || c == 'n') nd.kind = K_STR; else { node = nd.elem; nd = nodes[node]; } }
+    if constexpr (EXT) {
+      if (nd.kind == K_STRARR) { if (c == '"') nd.kind = K_STR; else if (c == '[') { node = nd.elem; nd = nodes[node]; } else return false; }
+      if (nd.kind == K_UNION) {   // the union's UnmarshalJSON: gjson "type", then json.Unmarshal into the variant
+        if (c != '{') return false;
+        int ts = 0, tl = 0; const int r = union_tag(p, i, n, ts, tl);
+        if (r == -2) { cap.weird = 1; return false; }
+        if (r <= 0) return false;
+        int v = -1;
+        for (int f = 0; f < nd.nf && v < 0; f++) {
+          const Field fd = fields[nd.f0 + f];
+          if (fd.klen == tl) { const char* fk = keys + fd.koff; int t = 0; while (t < tl && p[ts + t] == (uint8_t)fk[t]) t++; if (t == tl) v = fd.node; }
+        }
+        if (v < 0) return false;   // unknown tag
+        node = v; nd = nodes[node];
+      }
+      if (nd.kind == K_DECLINE) { cap.weird = 1; return false; }
+      if (nd.kind == K_PCREATED) nd.kind = c == 'n' ? K_ANY : K_CREATED;
+      if (nd.kind == K_F32) {
+        nd.kind = K_FLOAT;
+        bool ii; int ie; const int j = (c == '-' || dig(c)) ? scan_number(p, i, n, ii, ie) : -1;
+        if (j >= 0) { bool ex = false; for (int k = ie; k < j; k++) ex |= (p[k] | 0x20) == 'e'; if (ex || ie - i - (c == '-') > 38) cap.weird = 1; }
+      }
+    }
     bool descend = false;
     if (nd.kind == K_ANY) {
       const int j = skip_any(p, i, n); if (j < 0) return false;
@@ -243,7 +300,14 @@ __device__ inline bool walk(const uint8_t* p, int n, const Node* nodes, const Fi
       int child = -1;
       for (int f = 0; f < par.nf; f++) {
         const Field fd = fields[par.f0 + f];
-        if (fd.klen == kl) { const char* fk = keys + fd.koff; int t = 0; while (t < kl && k[t] == (uint8_t)fk[t]) t++; if (t == kl) { child = fd.node; if (st_seen[sp - 1] & (1u << f)) cap.weird = 1; st_seen[sp - 1] |= 1u << f; break; } }
+        if (fd.klen == kl) {
+          const char* fk = keys + fd.koff; int t = 0; while (t < kl && k[t] == (uint8_t)fk[t]) t++;
+          if (t == kl) {   // a repeated member decodes again; only the first 32 members of an object are tracked (EXT schemas order the captured ones first)
+            child = fd.node; const uint32_t bit = (EXT && f >= 32) ? 0u : 1u << f;
+            if (st_seen[sp - 1] & bit) cap.weird = 1;
+            st_seen[sp - 1] |= bit; break;
+          }
+        }
       }
       if (par.kind == K_MAP) child = par.elem;
       node = child < 0 ? 0 /* node 0 is K_ANY by convention */ : child;

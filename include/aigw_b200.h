@@ -238,6 +238,15 @@ int aigw_completions_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodie
                                            aigw_sse_result* d_results, void* stream, float* kernel_ms);
 int aigw_completions_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
                                          aigw_sse_result* results, const int32_t* cost_types, uint32_t n_costs, uint64_t* costs /* n * n_costs, may be NULL */);
+/* Same for /v1/responses: openAIToOpenAITranslatorV1Responses.ResponseBody, buffered branch (internal/translator/openai_responses.go:117-142)
+ * — json.NewDecoder(body).Decode(&openai.Response{}): the first JSON value counts and trailing bytes are ignored; an empty or
+ * white-space-only body is AIGW_INTERNAL.  model_len == 0 ⇒ the caller falls back to the request model (cmp.Or).  A non-null usage
+ * sets all six counters (uint32 of the int64 value, cache_creation from input_tokens_details.cache_creation_input_tokens); a null or
+ * absent usage sets none.  Output items, tools and tool choices outside the restated subset (DESIGN.md §4.3) are AIGW_DECLINED. */
+int aigw_responses_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
+                                         aigw_sse_result* d_results, void* stream, float* kernel_ms);
+int aigw_responses_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
+                                       aigw_sse_result* results, const int32_t* cost_types, uint32_t n_costs, uint64_t* costs /* n * n_costs, may be NULL */);
 int aigw_usage_costs_device(aigw_ctx* ctx, const aigw_sse_result* d_results, uint32_t n, const int32_t* d_cost_types, uint32_t n_costs,
                             uint64_t* d_costs, void* stream);
 
@@ -305,6 +314,13 @@ int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, 
  *                                    "event: <type>\ndata: <decoded bytes>\n\n" and reflected into the usage (message_start / message_delta,
  *                                    totals at eos), one that does not is dropped; message_start with content blocks, non-integer counts,
  *                                    web_search_tool_result blocks and escaped member names DECLINE.
+ *   AIGW_STREAM_OPENAI_RESPONSES     /v1/responses passthrough (openai_responses.go:102-114,146-192): usage scan, body UNCHANGED.  The
+ *                                    reference keeps NO carry: each call splits only its own bytes into lines (a line cut across calls
+ *                                    is lost; the last line is parsed without a newline), so the call's bytes are read in place, carry_len
+ *                                    is always 0 and the 15.6 KB carry limit does not apply.  response.created sets the stream's model,
+ *                                    response.completed sets all six counters (cache_creation 0; the call's last one wins); responseModel
+ *                                    = the stream's model, else the request's.  Output items / tools outside the restated subset, escaped
+ *                                    tags or models, and a response.completed without usage (the reference panics) DECLINE.
  *   AIGW_STREAM_GCP_GEMINI_BUFFERED  buffered GenerateContentResponse → ChatCompletionResponse (openai_gcpvertexai.go:139-198): feed the
  *                              body (≤ 15.6 KB) and set eos on the last call; the usage record is the call's `usage`
  * aigw_stream_chunks processes one ResponseBody call for each of n streams in ONE batch (a stream may appear once per call;
@@ -317,7 +333,8 @@ int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, 
  * cfg strings must not need JSON escaping (printable ASCII without '"' and '\\', ≤ 160 bytes), else -2. */
 enum aigw_stream_kind { AIGW_STREAM_OPENAI = 0, AIGW_STREAM_AWS_BEDROCK = 1, AIGW_STREAM_GCP_ANTHROPIC = 2, AIGW_STREAM_GCP_GEMINI = 3, AIGW_STREAM_GCP_GEMINI_BUFFERED = 4,
                         AIGW_STREAM_ANTHROPIC = 5, AIGW_STREAM_AWS_ANTHROPIC = 6, AIGW_STREAM_OPENAI_COMPLETIONS = 7,
-                        AIGW_STREAM_MESSAGES_OPENAI = 8, AIGW_STREAM_MESSAGES_OPENAI_BUFFERED = 9, AIGW_STREAM_MESSAGES_AWS_ANTHROPIC = 10 };
+                        AIGW_STREAM_MESSAGES_OPENAI = 8, AIGW_STREAM_MESSAGES_OPENAI_BUFFERED = 9, AIGW_STREAM_MESSAGES_AWS_ANTHROPIC = 10,
+                        AIGW_STREAM_OPENAI_RESPONSES = 11 };
 typedef struct aigw_stream_cfg { int32_t kind; int32_t _pad; int64_t created; const char* request_model; const char* response_id; } aigw_stream_cfg;
 typedef struct aigw_chunk_in { uint64_t handle; const uint8_t* bytes; uint32_t len; uint32_t eos; } aigw_chunk_in;
 typedef struct aigw_chunk_result {

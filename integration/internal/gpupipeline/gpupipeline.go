@@ -102,7 +102,8 @@ type Stream struct {
 
 // StreamKindFor maps the translator a route selected (endpoint + backend schema, internal/filterapi APISchemaName) to the library's
 // stream kind, or -1 when that response direction has no GPU path and the stock translator keeps handling the stream.
-// endpoint is the router filter's path family ("chat", "completions", "messages"); buffered selects the whole-body form where one exists.
+// endpoint is the router filter's path family ("chat", "completions", "messages", "responses"); buffered selects the whole-body form where
+// one exists.  A buffered /v1/responses body has no stream kind: its usage comes from aigw_responses_response_usage_host.
 func StreamKindFor(endpoint, backendSchema string, buffered bool) int {
 	switch endpoint {
 	case "chat":
@@ -124,6 +125,10 @@ func StreamKindFor(endpoint, backendSchema string, buffered bool) int {
 	case "completions":
 		if backendSchema == "OpenAI" || backendSchema == "AzureOpenAI" {
 			return C.AIGW_STREAM_OPENAI_COMPLETIONS // usage scan (openai_completions.go:80-203)
+		}
+	case "responses":
+		if backendSchema == "OpenAI" && !buffered {
+			return C.AIGW_STREAM_OPENAI_RESPONSES // usage scan without carry between calls (openai_responses.go:102-192)
 		}
 	case "messages":
 		switch backendSchema {

@@ -18,7 +18,7 @@ static void hex(const uint8_t* p, size_t n) { if (!n) { printf("-"); return; } f
 
 int main() {
   g_chunk_schema = build_schema(); g_cmpl_schema = build_completion_schema(); g_o2a_resp_schema = build_resp_schema();
-  g_conv_schema = build_schema_bedrock(); g_an_schema = build_an_schema();
+  g_conv_schema = build_schema_bedrock(); g_an_schema = build_an_schema(); g_rsp_schema = build_responses_schema();
   for (uint32_t i = 0; i < 256; i++) { uint32_t v = i; for (int k = 0; k < 8; k++) v = (v & 1u) ? 0xEDB88320u ^ (v >> 1) : v >> 1; g_crc_tab[i] = v; }
   StreamSlot* S = new StreamSlot();
   std::vector<uint8_t> out(1 << 22);
@@ -35,6 +35,14 @@ int main() {
     } else if (cmd == "feed") {
       std::string h; int eos; std::cin >> h >> eos; if (h == "-") h.clear();
       std::vector<uint8_t> in = unhex(h);
+      if (S->kind == AIGW_STREAM_OPENAI_RESPONSES) {   // no carry: stream_append_kernel leaves the slot alone, the step reads the call's bytes
+        aigw_chunk_result R; memset(&R, 0, sizeof R);
+        StreamStep st{0, (uint32_t)in.size(), (uint32_t)eos, (uint32_t)(16 * in.size() + 1024), 0, 0};
+        if (S->flags & SF_DEAD) R.status = (uint8_t)S->dead_status; else step_openai_responses(*S, st, in.data(), out.data(), R);
+        printf("%d %d %u %u %u %u %u %u %u %u ", (int)R.status, (int)R.body_kind, S->end - S->beg, R.usage.input, R.usage.output, R.usage.total, R.usage.cached, R.usage.cache_creation, R.usage.reasoning, R.usage.mask);
+        hex(out.data() + R.out_len, R.model_len); printf(" "); hex(out.data(), R.out_len); printf("\n");
+        continue;
+      }
       // stream_append_kernel: compact [beg, end) to the front, append the chunk
       const uint32_t keep = S->end - S->beg;
       memmove(S->buf, S->buf + S->beg, keep); S->beg = 0; S->end = keep;
