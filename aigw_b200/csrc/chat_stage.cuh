@@ -32,6 +32,17 @@ __device__ __forceinline__ uint32_t ctl_msb(uint32_t w, uint32_t z) { return ~((
 // msb mask → 4-bit mask (byte k → bit k): the four products land on bits 28..31 without carries
 __device__ __forceinline__ uint32_t nib_from_msb(uint32_t t) { return (t * 0x00204081u) >> 28; }
 
+// the four bytes s[p .. p+4) are hex digits; s is 4-byte aligned shared memory readable up to s[(p & ~3) + 8).  Two aligned word
+// reads and a per-byte range test ('0'..'9', or 'a'..'f' after folding case) instead of four dependent byte loads.
+__device__ __forceinline__ bool hex4_at(const uint8_t* s, uint32_t p) {
+  const uint32_t* w = (const uint32_t*)(s + (p & ~3u));
+  const uint32_t x = __funnelshift_r(w[0], w[1], (p & 3u) * 8u);
+  const uint32_t z = x & 0x7f7f7f7fu, l = z | 0x20202020u;
+  const uint32_t dig = (z + 0x50505050u) & ~(z + 0x46464646u);   // bit 7 of each byte: 0x30 <= z <= 0x39
+  const uint32_t let = (l + 0x1f1f1f1fu) & ~(l + 0x19191919u);   // 0x61 <= l <= 0x66
+  return ((dig | let) & ~x & 0x80808080u) == 0x80808080u;
+}
+
 // A round's sparse work (bytes outside strings, token compaction) is done cooperatively when few lanes own any of it:
 // the owning lane's mask is broadcast and lane i handles its bit i, so a 28-byte cluster of punctuation between two
 // messages costs one pass of ~12 instructions instead of a 28-trip single-lane loop.
@@ -103,11 +114,16 @@ __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len,
     // ps: bit set from an opening quote up to the byte before its closing quote
     if (mctl & ps) flags |= 1u;
     {  // escaped characters: \" \\ \n \r \t are what the encoder writes back; \/ \b \f \uXXXX are valid but re-spelled (marked per
-       // 32-byte block, re-escaped by the walk when the string is echoed); anything else is not JSON
+       // 32-byte block, re-escaped by the walk when the string is echoed); anything else is not JSON.  The four hex digits of \u are
+       // checked here: the walk decodes only the strings it echoes or looks up, and a key it skips must still be valid JSON
       uint32_t e = esc & ps; bool nc = false;
       while (e) {
-        const int j = __ffs(e) - 1; e &= e - 1; const uint32_t c = s_in[base + j];
-        if (!(c == '"' || c == '\\' || c == 'n' || c == 'r' || c == 't')) { if (c == '/' || c == 'b' || c == 'f' || c == 'u') nc = true; else flags |= 2u; }
+        const int j = __ffs(e) - 1; e &= e - 1; const uint32_t p = base + j, c = s_in[p];
+        if (!(c == '"' || c == '\\' || c == 'n' || c == 'r' || c == 't')) {
+          if (c == '/' || c == 'b' || c == 'f') nc = true;
+          else if (c == 'u' && p + 4u < len && hex4_at(s_in, p + 1)) nc = true;
+          else flags |= 2u;
+        }
       }
       const uint32_t ncm = __ballot_sync(FULL, nc);
       if (lane == 0) s_nc[r] = ncm;
