@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libaigw_b200.so")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
-SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
+SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_walk_g10.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "chat_small_g10.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
 
 
 def nvcc():

@@ -108,6 +108,50 @@ static_assert(MK_COUNT <= 64, "ids are 6 bits in the token word");
   X("name", MK_name) X("input", MK_input) X("tool_use_id", MK_tool_use_id) X("is_error", MK_is_error) X("description", MK_description) X("input_schema", MK_input_schema) \
   X("properties", MK_properties) X("required", MK_required) X("disable_parallel_tool_use", MK_disable_parallel_tool_use)
 
+// /v1/responses requests (P.schema & AIGW_SCHEMA_RESPONSES): the members of openai.ResponseRequest and of the input items, content
+// parts, tools, tool_choice and text.format the restated subset type-checks (internal/apischema/openai/openai.go:2183-2400,
+// 2415-2560, 2780-2792, 3477-3560, 3888-4130, 4784-4820, 4977-5014, 5634-5639).  RQK_DECL: a member the decoder knows that the
+// subset does not restate (the body declines).  Every other key has id 0 and is skipped, as the decoder ignores unknown fields.
+enum RQKid : uint8_t {
+  RQK_NONE = 0,
+  RQK_model, RQK_input, RQK_instructions, RQK_stream, RQK_background, RQK_parallel_tool_calls, RQK_store, RQK_max_output_tokens, RQK_max_tool_calls,
+  RQK_top_logprobs, RQK_temperature, RQK_top_p, RQK_presence_penalty, RQK_frequency_penalty, RQK_previous_response_id, RQK_prompt_cache_key,
+  RQK_safety_identifier, RQK_user, RQK_prompt_cache_retention, RQK_service_tier, RQK_truncation, RQK_include, RQK_metadata, RQK_conversation,
+  RQK_stream_options, RQK_reasoning, RQK_text, RQK_tool_choice, RQK_tools, RQK_DECL,
+  RQK_id, RQK_type, RQK_role, RQK_content, RQK_status, RQK_name, RQK_arguments, RQK_call_id, RQK_output, RQK_summary, RQK_encrypted_content,
+  RQK_annotations, RQK_logprobs, RQK_refusal, RQK_detail, RQK_file_id, RQK_image_url, RQK_file_data, RQK_file_url, RQK_filename,
+  RQK_include_obfuscation, RQK_effort, RQK_generate_summary, RQK_verbosity, RQK_format, RQK_schema, RQK_strict, RQK_description, RQK_parameters, RQK_COUNT
+};
+static_assert(RQK_COUNT <= 64, "ids are 6 bits in the token word");
+// insertion order: the keys of the input items first (the most looked-up ones sit nearest their home slot), then by length; this
+// order keeps every key within 6 probes of its home slot
+#define AIGW_RQKEYS(X) \
+  X("type", RQK_type) X("role", RQK_role) X("content", RQK_content) X("text", RQK_text) X("id", RQK_id) X("call_id", RQK_call_id) X("name", RQK_name) \
+  X("arguments", RQK_arguments) X("output", RQK_output) X("encrypted_content", RQK_encrypted_content) X("summary", RQK_summary) \
+  X("status", RQK_status) X("model", RQK_model) X("input", RQK_input) X("user", RQK_user) X("store", RQK_store) X("top_p", RQK_top_p) \
+  X("tools", RQK_tools) X("stream", RQK_stream) X("prompt", RQK_DECL) X("detail", RQK_detail) X("effort", RQK_effort) X("format", RQK_format) \
+  X("schema", RQK_schema) X("strict", RQK_strict) X("include", RQK_include) X("refusal", RQK_refusal) X("file_id", RQK_file_id) \
+  X("metadata", RQK_metadata) X("logprobs", RQK_logprobs) X("file_url", RQK_file_url) X("filename", RQK_filename) X("reasoning", RQK_reasoning) \
+  X("image_url", RQK_image_url) X("file_data", RQK_file_data) X("verbosity", RQK_verbosity) X("background", RQK_background) \
+  X("truncation", RQK_truncation) X("parameters", RQK_parameters) X("temperature", RQK_temperature) X("tool_choice", RQK_tool_choice) \
+  X("annotations", RQK_annotations) X("description", RQK_description) X("instructions", RQK_instructions) X("top_logprobs", RQK_top_logprobs) \
+  X("service_tier", RQK_service_tier) X("conversation", RQK_conversation) X("max_tool_calls", RQK_max_tool_calls) \
+  X("stream_options", RQK_stream_options) X("presence_penalty", RQK_presence_penalty) X("prompt_cache_key", RQK_prompt_cache_key) \
+  X("generate_summary", RQK_generate_summary) X("max_output_tokens", RQK_max_output_tokens) X("frequency_penalty", RQK_frequency_penalty) \
+  X("safety_identifier", RQK_safety_identifier) X("context_management", RQK_DECL) X("parallel_tool_calls", RQK_parallel_tool_calls) \
+  X("include_obfuscation", RQK_include_obfuscation) X("previous_response_id", RQK_previous_response_id) \
+  X("prompt_cache_retention", RQK_prompt_cache_retention)
+// the tags the walk compares (input items, content parts, tools, tool_choice, text.format) and the role that picks the output message
+enum RQVid : uint8_t {
+  RQV_NONE = 0, RQV_message, RQV_function_call, RQV_function_call_output, RQV_reasoning, RQV_item_reference, RQV_input_text, RQV_input_image,
+  RQV_input_file, RQV_output_text, RQV_refusal, RQV_function, RQV_text, RQV_json_object, RQV_json_schema, RQV_assistant
+};
+#define AIGW_RQVALS(X) \
+  X("message", RQV_message) X("function_call", RQV_function_call) X("function_call_output", RQV_function_call_output) X("reasoning", RQV_reasoning) \
+  X("item_reference", RQV_item_reference) X("input_text", RQV_input_text) X("input_image", RQV_input_image) X("input_file", RQV_input_file) \
+  X("output_text", RQV_output_text) X("refusal", RQV_refusal) X("function", RQV_function) X("text", RQV_text) X("json_object", RQV_json_object) \
+  X("json_schema", RQV_json_schema) X("assistant", RQV_assistant)
+
 static constexpr int kKeySlots = 128, kValSlots = 32, kMaxIdLen = 28, kIdWords = 7;
 // slot = { seven little-endian words of the string zero-padded to 28 bytes, len | id << 8 }
 struct IdSlot { uint32_t w[kIdWords]; uint32_t meta; };
@@ -169,6 +213,18 @@ constexpr IdTables make_msg_id_tables() {
 }
 static_assert(id_max_probe(make_msg_id_tables().key, kKeySlots) <= 6 && id_max_probe(make_msg_id_tables().val, kValSlots) <= 6, "messages id hash table needs more than 6 probes");
 static __device__ __constant__ IdTables c_ids_msg = make_msg_id_tables();
+constexpr IdTables make_rq_id_tables() {
+  IdTables t{};
+#define X(lit, idv) id_insert(t.key, kKeySlots, lit, idv);
+  AIGW_RQKEYS(X)
+#undef X
+#define X(lit, idv) id_insert(t.val, kValSlots, lit, idv);
+  AIGW_RQVALS(X)
+#undef X
+  return t;
+}
+static_assert(id_max_probe(make_rq_id_tables().key, kKeySlots) <= 6 && id_max_probe(make_rq_id_tables().val, kValSlots) <= 6, "responses id hash table needs more than 6 probes");
+static __device__ __constant__ IdTables c_ids_rq = make_rq_id_tables();
 
 // id of a short string (1 ≤ n ≤ kMaxIdLen) held in shared memory, against the key or the value table (also in shared
 // memory).  Straight-line code: seven aligned word loads, funnel shifts, length mask, multiplicative hash, ≤ 4 probes.

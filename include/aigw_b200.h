@@ -82,7 +82,24 @@ enum aigw_schema { AIGW_SCHEMA_OPENAI = 0, AIGW_SCHEMA_AWS_BEDROCK = 1, AIGW_SCH
                     * (internal/translator/anthropic_openai.go:55-93 + openai_helper.go:27-261; openai_prefix as for chat) and AWS Bedrock
                     * Converse (anthropic_awsbedrock.go:52-163,176-395).  Subset: text / tool_use / tool_result blocks, string or
                     * text-block system prompt, sampling parameters, stop sequences, custom tools, tool_choice; the rest is DECLINED. */
-                   AIGW_SCHEMA_MSG_OPENAI = 64, AIGW_SCHEMA_MSG_AWS_BEDROCK = 65 };
+                   AIGW_SCHEMA_MSG_OPENAI = 64, AIGW_SCHEMA_MSG_AWS_BEDROCK = 65,
+                   /* /v1/responses requests: ResponsesEndpointSpec.ParseBody (endpointspec.go:292-301, json.Unmarshal into
+                    * openai.ResponseRequest) + openAIToOpenAITranslatorV1Responses.RequestBody (openai_responses.go:50-78).
+                    * AIGW_SCHEMA_RESPONSES | base schema; only the OpenAI base has a translator (GetTranslator, endpointspec.go:304-311),
+                    * every other base is DECLINED (AIGW_R_SCHEMA).  Result as for the chat passthrough: model span = ParseBody's model,
+                    * flags bit0 = stream, record = [":path" = path.Join("/", openai_prefix, "responses")][body]; body_kind UNCHANGED, or
+                    * BYTES with model_name_override (sjson set of "model": the first value spliced, or the member appended at the root)
+                    * or force_body_mutation (the original bytes).  Restated subset, every member type-checked as the decoder does (a type
+                    * error is AIGW_MALFORMED_400, unknown keys are skipped): the scalar members, include, metadata, conversation (string or
+                    * {id}), stream_options, reasoning, text (verbosity; format text / json_object / json_schema), tool_choice (a string or
+                    * {type:"function", name}), tools (function tools), and input as a string or a list of: messages without a type, the
+                    * three resolutions of "message" (input, easy, assistant output message with output_text / refusal parts),
+                    * function_call, function_call_output with a string output, reasoning (summary, encrypted_content) and item_reference;
+                    * content parts input_text / input_image / input_file (strings type-checked only).  DECLINED: every other item, part,
+                    * tool or tool_choice tag (known or not), a null or non-object where a tagged union is decoded, prompt,
+                    * context_management, non-empty annotations / logprobs, escaped keys, tags and model, repeated restated keys, a null
+                    * root, float32 members with an exponent or more than 38 integer digits. */
+                   AIGW_SCHEMA_RESPONSES = 128, AIGW_SCHEMA_RESPONSES_OPENAI = 128 };
 
 /* Why a body was declined / rejected (diagnostics; stable numbering). */
 enum aigw_reason {

@@ -130,6 +130,7 @@ func StreamKindFor(endpoint, backendSchema string, buffered bool) int {
 		if backendSchema == "OpenAI" && !buffered {
 			return C.AIGW_STREAM_OPENAI_RESPONSES // usage scan without carry between calls (openai_responses.go:102-192)
 		}
+		// the request of the same route: ResponsesRequestSchema
 	case "messages":
 		switch backendSchema {
 		case "Anthropic", "GCPAnthropic":
@@ -142,6 +143,16 @@ func StreamKindFor(endpoint, backendSchema string, buffered bool) int {
 			}
 			return C.AIGW_STREAM_MESSAGES_OPENAI // OpenAI SSE -> Anthropic SSE (openai_helper.go:436-766)
 		}
+	}
+	return -1
+}
+
+// ResponsesRequestSchema is the aigw_backend_cfg.schema of a /v1/responses request to a backend of that schema (aigw_chat_translate_*
+// or the batcher: ResponsesEndpointSpec.ParseBody + RequestBody, endpointspec.go:292-311), or -1 when the backend has no translator
+// for the endpoint (GetTranslator serves only OpenAI) and the stock path reports that error.
+func ResponsesRequestSchema(backendSchema string) int {
+	if backendSchema == "OpenAI" {
+		return C.AIGW_SCHEMA_RESPONSES_OPENAI
 	}
 	return -1
 }
