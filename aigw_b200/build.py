@@ -7,7 +7,14 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libaigw_b200.so")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
-SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_walk_g10.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "chat_small_g10.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
+# Per-unit ptxas flags.  ptxas -O2 / -O3 of CUDA 12.9 (V12.9.86) miscompiles the straddling-chunk loop of emit_doc
+# (chat_stage.cuh) in the fused group-11 kernel.  The PTX is right: `add.s32 %k, %k, 1; … ld.shared.u32 [4*%k + s + 13632]`
+# reloads s_ops[k] after ++k.  The -O3 SASS increments k and then loads 4 bytes further:
+#     VIADD R23, R23, 0x1 ; IMAD R30, R23, 0x4, R20 ; LDS R26, [R30+0x3544]     (s_ops is at +0x3540: this is s_ops[k + 1])
+# so every chunk that spans two copy ops skips the second one.  At -O1 the reload is `LDS [R+0x3540]` and the bytes match the
+# oracle.  No other fused kernel (groups 0-10, built at -O3) contains the +0x3544 reload.  Cost of -O1 on this kernel: DESIGN.md §4.1.
+PTXAS = {"chat_small_g11.cu": ["-Xptxas", "-O1"]}
+SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_walk_g10.cu", "chat_walk_g11.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "chat_small_g10.cu", "chat_small_g11.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
 
 
 def nvcc():
@@ -42,7 +49,7 @@ def build(force=False, verbose=False):
         obj = os.path.join(objdir, src.replace(".cu", ".o"))
         path = os.path.join(CSRC, src)
         if force or not os.path.exists(obj) or os.path.getmtime(obj) < max(os.path.getmtime(path), hdr_t):
-            cmd = base + ["-c", path, "-o", obj]
+            cmd = base + PTXAS.get(src, []) + ["-c", path, "-o", obj]
             if verbose:
                 print(" ".join(cmd), file=sys.stderr)
             subprocess.check_call(cmd)

@@ -152,6 +152,20 @@ enum RQVid : uint8_t {
   X("output_text", RQV_output_text) X("refusal", RQV_refusal) X("function", RQV_function) X("text", RQV_text) X("json_object", RQV_json_object) \
   X("json_schema", RQV_json_schema) X("assistant", RQV_assistant)
 
+// /v1/completions requests (P.schema & AIGW_SCHEMA_COMPLETIONS): the members of openai.CompletionRequest
+// (internal/apischema/openai/openai.go:1883-1995) and StreamOptions.include_usage.  No value ids: the walk compares no strings.
+enum CPKid : uint8_t {
+  CPK_NONE = 0,
+  CPK_model, CPK_prompt, CPK_best_of, CPK_echo, CPK_frequency_penalty, CPK_logit_bias, CPK_logprobs, CPK_max_tokens, CPK_n, CPK_presence_penalty,
+  CPK_seed, CPK_stop, CPK_stream, CPK_stream_options, CPK_suffix, CPK_temperature, CPK_top_p, CPK_user, CPK_include_usage, CPK_COUNT
+};
+static_assert(CPK_COUNT <= 32, "the walk keeps the seen members in one 32-bit mask");
+#define AIGW_CPKEYS(X) \
+  X("model", CPK_model) X("prompt", CPK_prompt) X("max_tokens", CPK_max_tokens) X("temperature", CPK_temperature) X("stream", CPK_stream) \
+  X("stop", CPK_stop) X("top_p", CPK_top_p) X("n", CPK_n) X("suffix", CPK_suffix) X("echo", CPK_echo) X("logprobs", CPK_logprobs) X("seed", CPK_seed) \
+  X("user", CPK_user) X("best_of", CPK_best_of) X("logit_bias", CPK_logit_bias) X("stream_options", CPK_stream_options) \
+  X("include_usage", CPK_include_usage) X("presence_penalty", CPK_presence_penalty) X("frequency_penalty", CPK_frequency_penalty)
+
 static constexpr int kKeySlots = 128, kValSlots = 32, kMaxIdLen = 28, kIdWords = 7;
 // slot = { seven little-endian words of the string zero-padded to 28 bytes, len | id << 8 }
 struct IdSlot { uint32_t w[kIdWords]; uint32_t meta; };
@@ -225,6 +239,15 @@ constexpr IdTables make_rq_id_tables() {
 }
 static_assert(id_max_probe(make_rq_id_tables().key, kKeySlots) <= 6 && id_max_probe(make_rq_id_tables().val, kValSlots) <= 6, "responses id hash table needs more than 6 probes");
 static __device__ __constant__ IdTables c_ids_rq = make_rq_id_tables();
+constexpr IdTables make_cp_id_tables() {
+  IdTables t{};
+#define X(lit, idv) id_insert(t.key, kKeySlots, lit, idv);
+  AIGW_CPKEYS(X)
+#undef X
+  return t;
+}
+static_assert(id_max_probe(make_cp_id_tables().key, kKeySlots) <= 6, "completions id hash table needs more than 6 probes");
+static __device__ __constant__ IdTables c_ids_cp = make_cp_id_tables();
 
 // id of a short string (1 ≤ n ≤ kMaxIdLen) held in shared memory, against the key or the value table (also in shared
 // memory).  Straight-line code: seven aligned word loads, funnel shifts, length mask, multiplicative hash, ≤ 4 probes.

@@ -181,11 +181,12 @@ static void fill_params(ChatParams& P, const aigw_backend_cfg* cfg) {
     size_t n = strlen(cfg->model_name_override); if (n > sizeof P.override_model) n = sizeof P.override_model;
     memcpy(P.override_model, cfg->model_name_override, n); P.override_len = (uint16_t)n;
   }
-  // path.Join("/", prefix, "chat/completions") (openai_openai.go:30), "embeddings", "responses" (openai_responses.go:52)
+  // path.Join("/", prefix, "chat/completions") (openai_openai.go:30), "embeddings", "responses" (openai_responses.go:52),
+  // "completions" (openai_completions.go:26)
   std::string pfx = (cfg && cfg->openai_prefix) ? cfg->openai_prefix : "v1";
   while (!pfx.empty() && pfx.front() == '/') pfx.erase(0, 1);
   while (!pfx.empty() && pfx.back() == '/') pfx.pop_back();
-  const char* endpoint = !cfg ? "chat/completions" : (cfg->schema & AIGW_SCHEMA_RESPONSES) ? "responses" : (cfg->schema & AIGW_SCHEMA_EMBEDDINGS) ? "embeddings" : "chat/completions";
+  const char* endpoint = !cfg ? "chat/completions" : (cfg->schema & AIGW_SCHEMA_COMPLETIONS) ? "completions" : (cfg->schema & AIGW_SCHEMA_RESPONSES) ? "responses" : (cfg->schema & AIGW_SCHEMA_EMBEDDINGS) ? "embeddings" : "chat/completions";
   std::string path = "/" + (pfx.empty() ? std::string() : pfx + "/") + endpoint;
   if (path.size() > sizeof P.openai_path) path.resize(sizeof P.openai_path);
   memcpy(P.openai_path, path.data(), path.size()); P.prefix_len = (uint16_t)path.size();

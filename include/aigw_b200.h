@@ -99,7 +99,23 @@ enum aigw_schema { AIGW_SCHEMA_OPENAI = 0, AIGW_SCHEMA_AWS_BEDROCK = 1, AIGW_SCH
                     * tool or tool_choice tag (known or not), a null or non-object where a tagged union is decoded, prompt,
                     * context_management, non-empty annotations / logprobs, escaped keys, tags and model, repeated restated keys, a null
                     * root, float32 members with an exponent or more than 38 integer digits. */
-                   AIGW_SCHEMA_RESPONSES = 128, AIGW_SCHEMA_RESPONSES_OPENAI = 128 };
+                   AIGW_SCHEMA_RESPONSES = 128, AIGW_SCHEMA_RESPONSES_OPENAI = 128,
+                   /* /v1/completions requests: CompletionsEndpointSpec.ParseBody (endpointspec.go:203-212, json.Unmarshal into
+                    * openai.CompletionRequest) + openAIToOpenAITranslatorV1Completion.RequestBody (openai_completions.go:44-67).
+                    * AIGW_SCHEMA_COMPLETIONS | base schema; only the OpenAI base has a translator (GetTranslator, endpointspec.go:215-222),
+                    * every other base is DECLINED (AIGW_R_SCHEMA).  Result as for the chat passthrough: model span = ParseBody's model,
+                    * flags bit0 = stream (bit1 never: ParseBody returns no mutated body), record = [":path" = path.Join("/",
+                    * openai_prefix, "completions")][body]; body_kind UNCHANGED, or BYTES with model_name_override (sjson set of "model")
+                    * or force_body_mutation (the original bytes).  Every member is type-checked as the decoder does (a type error is
+                    * AIGW_MALFORMED_400, unknown keys are skipped, ranges are not checked): model / suffix / user strings, echo / stream
+                    * bools, best_of / logprobs / max_tokens / n / seed int64 (exact range; a fraction or exponent is a 400),
+                    * frequency_penalty / presence_penalty / temperature / top_p float64, logit_bias (object of ints), stop (any JSON
+                    * value; its numbers decode as float64), stream_options ({include_usage: bool}), and prompt as a string, [], or an array whose first element picks
+                    * []string / [][]int64 / []int64 (null elements allowed; a first element that is null, an object or a bool is a 400).
+                    * DECLINED: a null root, "prompt":null, escaped keys and model, repeated known keys, float64 values (members, numbers
+                    * in stop) with an exponent or more than 308 integer digits.  A token-id prompt costs two index tokens per id, so long ones decline with
+                    * AIGW_R_TOKENS (DESIGN.md §7). */
+                   AIGW_SCHEMA_COMPLETIONS = 256, AIGW_SCHEMA_COMPLETIONS_OPENAI = 256 };
 
 /* Why a body was declined / rejected (diagnostics; stable numbering). */
 enum aigw_reason {

@@ -126,6 +126,7 @@ func StreamKindFor(endpoint, backendSchema string, buffered bool) int {
 		if backendSchema == "OpenAI" || backendSchema == "AzureOpenAI" {
 			return C.AIGW_STREAM_OPENAI_COMPLETIONS // usage scan (openai_completions.go:80-203)
 		}
+		// the request of the same route: CompletionsRequestSchema
 	case "responses":
 		if backendSchema == "OpenAI" && !buffered {
 			return C.AIGW_STREAM_OPENAI_RESPONSES // usage scan without carry between calls (openai_responses.go:102-192)
@@ -153,6 +154,16 @@ func StreamKindFor(endpoint, backendSchema string, buffered bool) int {
 func ResponsesRequestSchema(backendSchema string) int {
 	if backendSchema == "OpenAI" {
 		return C.AIGW_SCHEMA_RESPONSES_OPENAI
+	}
+	return -1
+}
+
+// CompletionsRequestSchema is the aigw_backend_cfg.schema of a /v1/completions request to a backend of that schema
+// (aigw_chat_translate_* or the batcher: CompletionsEndpointSpec.ParseBody + RequestBody, endpointspec.go:203-222), or -1 when the
+// backend has no translator for the endpoint (GetTranslator serves only OpenAI) and the stock path reports that error.
+func CompletionsRequestSchema(backendSchema string) int {
+	if backendSchema == "OpenAI" {
+		return C.AIGW_SCHEMA_COMPLETIONS_OPENAI
 	}
 	return -1
 }
