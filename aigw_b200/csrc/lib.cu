@@ -10,6 +10,7 @@
 #include <memory>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "chat_kernel.cuh"
@@ -97,12 +98,8 @@ struct aigw_ctx {
   PinnedScratch<uint8_t> h_out;
   PinnedScratch<aigw_doc_result> h_res;
   long small_max = -1;   // aigw_chat_set_small_batch; -1: AIGW_SMALL_MAX or 512
-  // BPE count (host form): device staging
-  Scratch<uint8_t> d_bpe_text; Scratch<uint64_t> d_bpe_off; Scratch<uint32_t> d_bpe_len; Scratch<uint32_t> d_bpe_cnt;
-  // large embeddings requests (aigw_embeddings_count_*): token workspace, text table, counts, host-form staging
-  Scratch<uint32_t> d_emb_tok; Scratch<uint64_t> d_emb_toff; Scratch<uint32_t> d_emb_tlen;
-  Scratch<uint32_t> d_emb_cnt; Scratch<uint8_t> d_emb_body; Scratch<uint64_t> d_emb_off;
-  Scratch<uint32_t> d_emb_len; Scratch<aigw_emb_count_result> d_emb_res;
+  // large embeddings requests (aigw_embeddings_count_device): token workspace, text table, counts
+  Scratch<uint32_t> d_emb_tok; Scratch<uint64_t> d_emb_toff; Scratch<uint32_t> d_emb_tlen; Scratch<uint32_t> d_emb_cnt;
   PinnedScratch<uint8_t> h_small;   // small-batch path: tables + bodies, read by the kernel in place
   // chat workspace (intermediates of one sub-batch) + per-stage timing events
   Scratch<uint8_t> d_work;
@@ -110,17 +107,9 @@ struct aigw_ctx {
   cudaEvent_t stage_ev[64]; float stage_ms[3] = {0, 0, 0}; int last_launches = 0;
   bool profile_stages = false;   // aigw_chat_set_profile: next device calls run the stages back to back on one stream and time them
   ChatAux aux{};                 // two extra streams: sub-batches of one call alternate between them
-  // device staging of the single-shot host calls (SSE usage, response usage, CEL costs, SHA-256); each call lays out its own
-  // tables in them, so their element types are only the common case
-  Scratch<uint8_t> stage_bytes;
-  Scratch<uint64_t> stage_off;
-  Scratch<uint32_t> stage_len;
-  Scratch<aigw_sse_result> stage_res;
-  // bedrock stream workspace (records + counts) and host-API buffers
-  Scratch<uint8_t> d_bs_work;
-  Scratch<uint64_t> d_bs_off[2];
-  PinnedScratch<aigw_stream_result> h_sres;
-  PinnedScratch<aigw_mut_result> h_mres;
+  Scratch<uint8_t> d_stage[6];   // HostStage: one buffer per input table or output area of a single-shot host call (six at most)
+  Scratch<uint8_t> d_bs_work;    // bedrock stream workspace (records + counts)
+  PinnedScratch<uint8_t> h_chunk_res;   // chunk_pipeline: the mapped result table
   std::vector<uint32_t> h_map;   // size-class bucketing scratch (host)
   // ---- stateful response streams (aigw_stream_*): device-resident slots + per-call staging
   struct StreamPool {
@@ -155,6 +144,53 @@ static int timed(aigw_ctx* ctx, cudaStream_t st, float* kernel_ms, F&& launch) {
   return 0;
 }
 
+// Staging of the single-shot host calls: each stages its inputs with in() / span(), takes its output areas with out(), runs its
+// *_device form on st, copies its outputs back with back() and ends with wait(): the call's one synchronisation, after which it
+// reports the bytes the call copied in and out.  Every table and output area of a call gets a d_stage buffer of its own, in the
+// order the call asks for them; no other call uses these buffers.  The first failure is kept in rc: later steps do nothing and
+// hand out null pointers, so a call checks rc once before its launch.
+struct HostStage {
+  aigw_ctx* const ctx;
+  const cudaStream_t st;
+  int rc = 0, next = 0;
+  uint64_t h2d = 0, d2h = 0;   // bytes copied in and out
+  explicit HostStage(aigw_ctx* c) : ctx(c), st(c->s_compute) {}
+
+  template <class F> void step(F&& f) { if (!rc) rc = f(); }
+  template <class T> T* out(size_t count) {   // 64 bytes of slack: kernels may read a little past a body
+    Scratch<uint8_t>& b = ctx->d_stage[next++];
+    step([&] { CK(b.ensure(count * sizeof(T) + 64)); return 0; });
+    return rc ? nullptr : (T*)b.p;
+  }
+  template <class T> const T* in(const T* host, size_t count) {
+    T* dev = out<T>(count);
+    step([&] { CK(cudaMemcpyAsync(dev, host, count * sizeof(T), cudaMemcpyHostToDevice, st)); return 0; });
+    h2d += count * sizeof(T);
+    return dev;
+  }
+  // Body i of a (bytes, offsets, lens) table is bytes[offsets[i] .. offsets[i]+lens[i]), in any order.  One copy of the span from the
+  // lowest start, rounded down to 16, to the highest end; the device pointer is rebased so that the offsets index it unchanged and
+  // every body keeps its alignment modulo 16.
+  const uint8_t* span(const uint8_t* bytes, const uint64_t* offsets, const uint32_t* lens, uint32_t n, uint64_t* span_bytes = nullptr) {
+    uint64_t lo = ~0ull, hi = 0;
+    for (uint32_t i = 0; i < n; i++) { if (offsets[i] < lo) lo = offsets[i]; if (offsets[i] + lens[i] > hi) hi = offsets[i] + lens[i]; }
+    lo &= ~15ull;
+    if (span_bytes) *span_bytes = hi - lo;
+    const uint8_t* dev = in(bytes + lo, hi - lo);
+    return rc ? nullptr : dev - lo;
+  }
+  template <class T> void back(T* host, const T* dev, size_t count) {
+    step([&] { CK(cudaMemcpyAsync(host, dev, count * sizeof(T), cudaMemcpyDeviceToHost, st)); return 0; });
+    d2h += count * sizeof(T);
+  }
+  int wait(uint64_t* h2d_bytes = nullptr, uint64_t* d2h_bytes = nullptr) {
+    step([&] { CK(cudaStreamSynchronize(st)); return 0; });
+    if (!rc && h2d_bytes) *h2d_bytes = h2d;
+    if (!rc && d2h_bytes) *d2h_bytes = d2h;
+    return rc;
+  }
+};
+
 // Pipeline chunks of the host calls: chunk c is documents [cb[c], cb[c+1]).  A chunk holds at least one document and ends before
 // the first document i with end(i) - start(first document of the chunk) > budget.
 template <class S, class E>
@@ -167,8 +203,21 @@ static std::vector<uint32_t> chunk_bounds(uint32_t n, uint64_t budget, S&& start
   return cb;
 }
 
-// response bodies expand (escaped tool arguments, configuration text): plan them in a roomier size class
-static uint32_t resp_class_len(uint32_t max_len) { uint64_t m = (uint64_t)max_len * 4; if (m < 5120) m = 5120; if (m > 65536) m = max_len > 65536u ? max_len : 65536u; return (uint32_t)m; }
+// response direction (AIGW_SCHEMA_RESP_*, any backend): the bodies are upstream responses
+static bool response_dir(const aigw_backend_cfg* cfg) { return cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK; }
+
+// the length a body is planned at: response bodies expand (escaped tool arguments, configuration text), so they get a roomier size class
+static uint32_t class_len(const aigw_backend_cfg* cfg, uint32_t len) {
+  if (!response_dir(cfg)) return len;
+  uint64_t m = (uint64_t)len * 4; if (m < 5120) m = 5120; if (m > 65536) m = len > 65536u ? len : 65536u; return (uint32_t)m;
+}
+
+// the buffers of one launch (out_bias: where `out` lies in the arena the records' out_off index)
+static void chat_buffers(ChatParams& P, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, uint8_t* out, uint64_t out_capacity,
+                         aigw_doc_result* results, unsigned long long* out_used, uint64_t out_bias, const uint32_t* doc_map) {
+  P.bodies = bodies; P.offsets = offsets; P.lens = lens; P.n = n; P.out = out; P.out_capacity = out_capacity;
+  P.results = results; P.out_used = out_used; P.next_doc = nullptr; P.out_bias = out_bias; P.doc_map = doc_map;
+}
 
 static void fill_params(ChatParams& P, const aigw_backend_cfg* cfg) {
   P.schema = cfg ? cfg->schema : AIGW_SCHEMA_OPENAI;
@@ -191,7 +240,7 @@ static void fill_params(ChatParams& P, const aigw_backend_cfg* cfg) {
   if (path.size() > sizeof P.openai_path) path.resize(sizeof P.openai_path);
   memcpy(P.openai_path, path.data(), path.size()); P.prefix_len = (uint16_t)path.size();
   P.created = 0; P.rid_len = 0; memset(P.response_id, 0, sizeof P.response_id);
-  if (cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK) {   // response direction (any backend)
+  if (response_dir(cfg)) {
     P.created = cfg->created;
     if (cfg->response_id) { size_t n = strlen(cfg->response_id); if (n > sizeof P.response_id) n = sizeof P.response_id; memcpy(P.response_id, cfg->response_id, n); P.rid_len = (uint16_t)n; }
   }
@@ -199,15 +248,11 @@ static void fill_params(ChatParams& P, const aigw_backend_cfg* cfg) {
 
 namespace aigw {
 int ctx_device(const aigw_ctx* ctx) { return ctx->device; }
-bool chat_small_fits(const aigw_backend_cfg* cfg, uint32_t len) {
-  const bool resp = cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK;
-  return len > 0 && (resp ? resp_class_len(len) : len) <= kSmallMaxLen;
-}
+bool chat_small_fits(const aigw_backend_cfg* cfg, uint32_t len) { return len > 0 && class_len(cfg, len) <= kSmallMaxLen; }
 cudaError_t chat_small_launch(const aigw_backend_cfg* cfg, const uint8_t* in, const uint64_t* offsets, const uint32_t* lens, const uint64_t* out_slot, uint32_t n, uint8_t* out,
                               aigw_doc_result* results, cudaStream_t st) {
   ChatParams P; fill_params(P, cfg);
-  P.bodies = in; P.offsets = offsets; P.lens = lens; P.n = n;
-  P.out = out; P.out_capacity = 0; P.results = results; P.out_used = nullptr; P.next_doc = nullptr; P.out_bias = 0; P.doc_map = nullptr;
+  chat_buffers(P, in, offsets, lens, n, out, 0, results, nullptr, 0, nullptr);
   return launch_chat_small(P, 0, n, out_slot, st);
 }
 }  // namespace aigw
@@ -222,6 +267,84 @@ static void host_parallel_for(uint32_t n, F&& f) {
   for (unsigned t = 1; t < hw; t++) { const uint32_t b = t * per, e = b + per < n ? b + per : n; if (b < e) th.emplace_back([&f, b, e] { f(b, e); }); }
   f(0u, per < n ? per : n);
   for (auto& x : th) x.join();
+}
+
+// One chunk of chunk_pipeline: items [first, first + n) of the call, staged in a slot.
+template <class R>
+struct PipeChunk {
+  uint32_t first, n;
+  const uint8_t* bytes;            // the staged input, indexed by the caller's offsets
+  const uint64_t* off;             // the staged offset table from item `first` on: n + 1 entries, or n with a length table
+  const uint32_t* len;             // the staged length table, or null
+  uint8_t* out; uint64_t out_cap;  // the chunk's part of the output arena (device view)
+  uint64_t out_bias;               // where that part starts in the arena: added to the records' out_off
+  unsigned long long* out_used;    // the chunk's bump counter, zeroed
+  R* results;                      // results of the chunk's items (device view)
+  uint64_t max_in; uint32_t max_n; // the largest chunk of the call: sizes a workspace the chunks share
+};
+
+// The host-buffer pipeline of aigw_bedrock_stream_host and aigw_body_mutate_host.  Item i is bytes[off[i] .. off[i+1]) (len null:
+// an n+1 offset table) or bytes[off[i] .. off[i]+len[i]) (bodies in arena order).  The items are cut into chunks of about `budget`
+// bytes that alternate between two slots: the H2D copy of chunk c+1 (s_h2d) overlaps the kernels of chunk c (s_compute), which
+// store the records and results straight into mapped pinned host memory; one synchronisation at the end.  out_cap(in_bytes, items)
+// is a chunk's output capacity; launch(chunk) starts `launches` kernels on s_compute.
+template <class Out, class Cap, class Launch>
+static int chunk_pipeline(aigw_ctx* ctx, const uint8_t* bytes, const uint64_t* off, const uint32_t* len, uint32_t n, uint64_t budget,
+                          Cap&& out_cap_of, uint32_t launches, Launch&& launch, Out* out) {
+  using R = std::remove_const_t<std::remove_pointer_t<decltype(out->results)>>;
+  auto end = [&](uint32_t i) { return len ? off[i] + len[i] : off[i + 1]; };
+  const std::vector<uint32_t> cb = chunk_bounds(n, budget, [&](uint32_t i) { return off[i]; }, end);
+  const int nch = (int)cb.size() - 1;
+  std::vector<uint64_t> in_bytes(nch), out_cap(nch), out_base(nch);
+  uint64_t max_in = 0, total_cap = 0; uint32_t max_n = 0;
+  for (int c = 0; c < nch; c++) {
+    const uint32_t b = cb[c], nd = cb[c + 1] - b;
+    in_bytes[c] = end(cb[c + 1] - 1) - off[b];
+    if (in_bytes[c] > max_in) max_in = in_bytes[c]; if (nd > max_n) max_n = nd;
+    out_cap[c] = out_cap_of(in_bytes[c], nd);
+    out_base[c] = total_cap; total_cap += out_cap[c];
+  }
+  const int nslots = nch < 2 ? 1 : 2;
+  for (int k = 0; k < nslots; k++) {
+    ChunkSlot& S = ctx->slot[k];
+    CK(S.d_in.ensure(max_in + 64));
+    CK(S.d_off.ensure(((size_t)max_n + 1) * 8));
+    if (len) CK(S.d_len.ensure((size_t)max_n * 4));
+  }
+  CK(ctx->h_out.ensure(total_cap));
+  CK(ctx->h_chunk_res.ensure((size_t)n * sizeof(R)));
+  CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
+  uint8_t* dev_out = nullptr; R* dev_res = nullptr;
+  CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0));
+  CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_chunk_res, 0));
+  uint64_t h2d = 0;
+  CK(cudaMemsetAsync(ctx->d_used_arr, 0, (size_t)nch * 8, ctx->s_compute));
+  CK(cudaEventRecord(ctx->ev0, ctx->s_compute));
+  for (int c = 0; c < nch; c++) {
+    ChunkSlot& S = ctx->slot[c % nslots];
+    const uint32_t b = cb[c], nd = cb[c + 1] - b;
+    const size_t n_off = len ? nd : (size_t)nd + 1;
+    if (c >= nslots) CK(cudaStreamWaitEvent(ctx->s_h2d, S.ev_k1, 0));   // the slot's input has been consumed
+    CK(cudaMemcpyAsync(S.d_in, bytes + off[b], in_bytes[c], cudaMemcpyHostToDevice, ctx->s_h2d));
+    CK(cudaMemcpyAsync(S.d_off, off + b, n_off * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
+    if (len) CK(cudaMemcpyAsync(S.d_len, len + b, (size_t)nd * 4, cudaMemcpyHostToDevice, ctx->s_h2d));
+    CK(cudaEventRecord(S.ev_h2d, ctx->s_h2d));
+    h2d += in_bytes[c] + n_off * 8 + (len ? (uint64_t)nd * 4 : 0);
+    CK(cudaStreamWaitEvent(ctx->s_compute, S.ev_h2d, 0));
+    if (int rc = launch(PipeChunk<R>{b, nd, S.d_in - off[b], S.d_off, len ? (const uint32_t*)S.d_len : nullptr, dev_out + out_base[c], out_cap[c], out_base[c],
+                                     ctx->d_used_arr + c, dev_res + b, max_in, max_n}))
+      return rc;
+    CK(cudaEventRecord(S.ev_k1, ctx->s_compute));
+    out->gpu_launches += launches;
+  }
+  CK(cudaEventRecord(ctx->ev1, ctx->s_compute));
+  CK(cudaMemcpyAsync(ctx->h_used_arr, ctx->d_used_arr, (size_t)nch * 8, cudaMemcpyDeviceToHost, ctx->s_compute));
+  CK(cudaStreamSynchronize(ctx->s_compute));
+  uint64_t d2h = (uint64_t)n * sizeof(R) + (uint64_t)nch * 8;
+  for (int c = 0; c < nch; c++) d2h += ctx->h_used_arr[c] < out_cap[c] ? ctx->h_used_arr[c] : out_cap[c];
+  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+  out->results = (const R*)ctx->h_chunk_res.p; out->out = ctx->h_out; out->out_used = total_cap; out->h2d_bytes = h2d; out->d2h_bytes = d2h; out->kernel_ms = ms;
+  return 0;
 }
 
 extern "C" {
@@ -318,6 +441,16 @@ int aigw_memcpy_d2h(aigw_ctx* ctx, void* dst, const void* src, size_t bytes) { E
 int aigw_memset_d(aigw_ctx* ctx, void* dst, int v, size_t bytes) { ENTER(); CK(cudaMemset(dst, v, bytes)); return 0; }
 int aigw_sync(aigw_ctx* ctx) { ENTER(); CK(cudaDeviceSynchronize()); return 0; }
 
+// the translate workspace for `docs` documents planned at max_len bytes: two sub-batches in flight (one per auxiliary stream;
+// profiling runs one large sub-batch at a time), at most 3 GiB: the launcher walks a size class in sub-batches that fit it
+static int ensure_chat_work(aigw_ctx* ctx, uint32_t max_len, uint32_t docs) {
+  size_t need = chat_work_bytes_for(max_len, docs);
+  const size_t cap = (size_t)3 << 30, floor1 = chat_work_bytes(max_len, 1024);
+  if (need > cap) need = cap > floor1 ? cap : floor1;
+  CK(ctx->d_work.ensure(need));
+  return 0;
+}
+
 static int chat_translate_device_impl(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
                                       const uint32_t* d_lens, const uint32_t* d_doc_map, uint32_t first, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
                                       aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
@@ -325,18 +458,10 @@ static int chat_translate_device_impl(aigw_ctx* ctx, const aigw_backend_cfg* cfg
   ENTER_ON(stream);
   ChatParams P;
   fill_params(P, cfg);
-  P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.out = d_out; P.out_capacity = out_capacity;
-  P.results = d_results; P.out_used = (unsigned long long*)d_out_used;
-  P.next_doc = nullptr; P.out_bias = 0; P.doc_map = d_doc_map;
-  uint32_t ml = max_len ? max_len : 65536u;
-  if (cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK) ml = resp_class_len(ml);
+  chat_buffers(P, d_bodies, d_offsets, d_lens, n, d_out, out_capacity, d_results, (unsigned long long*)d_out_used, 0, d_doc_map);
+  const uint32_t ml = class_len(cfg, max_len ? max_len : 65536u);
   const bool stages = ctx->profile_stages && kernel_ms;
-  {  // workspace: two sub-batches in flight (one per auxiliary stream); profiling runs one large sub-batch at a time
-    size_t need = chat_work_bytes_for(ml, n);
-    const size_t cap = (size_t)3 << 30, floor1 = chat_work_bytes(ml, 1024);
-    if (need > cap) need = cap > floor1 ? cap : floor1;
-    CK(ctx->d_work.ensure(need));
-  }
+  if (int rc = ensure_chat_work(ctx, ml, n)) return rc;
   if (int rc = timed(ctx, st, kernel_ms, [&] {
         CK(launch_chat_translate(P, ml, ctx->device, ctx->sm_count, st, ctx->d_work, ctx->d_work.cap, &ctx->aux, &ctx->last_launches, stages ? ctx->stage_ev : nullptr, 64, first));
         return 0;
@@ -394,8 +519,7 @@ static int chat_small_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uin
   uint8_t* d_small = nullptr; uint8_t* d_out = nullptr; aigw_doc_result* d_res = nullptr;
   CK(cudaHostGetDevicePointer((void**)&d_small, ctx->h_small, 0)); CK(cudaHostGetDevicePointer((void**)&d_out, ctx->h_out, 0)); CK(cudaHostGetDevicePointer((void**)&d_res, ctx->h_res, 0));
   ChatParams P; fill_params(P, cfg);
-  P.bodies = d_small + tab; P.offsets = (const uint64_t*)d_small; P.lens = (const uint32_t*)(d_small + ((size_t)n + 1) * 16); P.n = n;
-  P.out = d_out; P.out_capacity = so; P.results = d_res; P.out_used = nullptr; P.next_doc = nullptr; P.out_bias = 0; P.doc_map = nullptr;
+  chat_buffers(P, d_small + tab, (const uint64_t*)d_small, (const uint32_t*)(d_small + ((size_t)n + 1) * 16), n, d_out, so, d_res, nullptr, 0, nullptr);
   static const bool dbg = getenv("AIGW_SMALL_DBG") != nullptr;
   static unsigned int* h_dbg = nullptr;
   if (dbg) { if (!h_dbg) cudaHostAlloc((void**)&h_dbg, 64, cudaHostAllocDefault); P.next_doc = h_dbg; }
@@ -428,9 +552,8 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   {
     static const long env_small_max = getenv("AIGW_SMALL_MAX") ? atol(getenv("AIGW_SMALL_MAX")) : 512;   // 0 disables the fused small-batch path
     if ((long)n <= (ctx->small_max >= 0 ? ctx->small_max : env_small_max)) {
-      const bool resp = cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK;
       uint32_t ml = 0; for (uint32_t i = 0; i < n; i++) if (lens[i] > ml) ml = lens[i];
-      if ((resp ? resp_class_len(ml) : ml) <= kSmallMaxLen) return chat_small_host(ctx, cfg, bodies, offsets, lens, n, out);
+      if (class_len(cfg, ml) <= kSmallMaxLen) return chat_small_host(ctx, cfg, bodies, offsets, lens, n, out);
     }
   }
   static const bool zero_copy = getenv("AIGW_HOST_ZEROCOPY") != nullptr;
@@ -457,18 +580,11 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     if (!zero_copy) CK(S.d_out.ensure(max_out + 64));
     CK(S.d_off.ensure((size_t)max_docs * 8)); CK(S.d_len.ensure((size_t)max_docs * 4)); CK(S.d_res.ensure((size_t)max_docs * sizeof(aigw_doc_result)));
   }
-  const bool resp_dir = cfg && (cfg->schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK;
-  if (resp_dir) max_len = resp_class_len(max_len);
+  max_len = class_len(cfg, max_len);
   // size classes (the kernels' shared-memory footprints, chat_kernel.cu launch_chat_translate)
   static const uint32_t kClsMax[6] = {2048, 5120, 9216, 17408, 33792, 65536};
-  auto cls_of = [&](uint32_t len) { const uint32_t l = resp_dir ? resp_class_len(len) : len; int k = 0; while (k < 5 && l > kClsMax[k]) k++; return k; };
-  {
-    size_t need = chat_work_bytes_for(max_len, max_docs);
-    const size_t cap = (size_t)3 << 30;   // the launcher walks a class in sub-batches that fit the workspace
-    const size_t floor1 = chat_work_bytes(max_len, 1024);
-    if (need > cap) need = cap > floor1 ? cap : floor1;
-    CK(ctx->d_work.ensure(need));
-  }
+  auto cls_of = [&](uint32_t len) { const uint32_t l = class_len(cfg, len); int k = 0; while (k < 5 && l > kClsMax[k]) k++; return k; };
+  if (int rc = ensure_chat_work(ctx, max_len, max_docs)) return rc;
   CK(ctx->h_out.ensure(total_out_cap));
   CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result)));
   CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
@@ -522,18 +638,16 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     CK(cudaEventRecord(S.ev_h2d, ctx->s_h2d));
     h2d += in_bytes[c] - 16 + (uint64_t)nd * 12;
     CK(cudaStreamWaitEvent(ctx->s_compute, S.ev_h2d, 0));
+    // documents keep their global index: kernels address offsets/lens/results with doc0 + i (or doc_map[i]), and the absolute
+    // offsets index straight into the chunk
     ChatParams P = P0;
-    P.bodies = S.d_in - offsets[b];  // absolute offsets index straight into the chunk
-    P.offsets = S.d_off - b; P.lens = S.d_len - b; P.n = nd;
-    P.out = zero_copy ? dev_out + out_base[c] : S.d_out; P.out_capacity = out_cap[c];
-    P.results = zero_copy ? dev_res : S.d_res - b; P.out_used = ctx->d_used_arr + c; P.next_doc = nullptr; P.out_bias = out_base[c]; P.doc_map = nullptr;
-    // documents keep their global index: kernels address offsets/lens/results with doc0 + i (or doc_map[i])
+    chat_buffers(P, S.d_in - offsets[b], S.d_off - b, S.d_len - b, nd, zero_copy ? dev_out + out_base[c] : S.d_out, out_cap[c],
+                 zero_copy ? dev_res : S.d_res - b, ctx->d_used_arr + c, out_base[c], n_cls > 1 ? (const uint32_t*)S.d_map : nullptr);
     if (n_cls <= 1) {
       int nl = 0;
       CK(launch_chat_translate_range(P, b, nd, kClsMax[top_cls], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &ctx->aux, &nl));
       out->gpu_launches += nl;
     } else {
-      P.doc_map = S.d_map;
       for (int k = 0; k < 6; k++) {
         if (!cls_cnt[k]) continue;
         int nl = 0;
@@ -596,23 +710,15 @@ int aigw_bpe_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t* text,
   if (!ctx || !bpe) return -2;
   if (n == 0) return 0;
   ENTER();
-  uint64_t nbytes = 0; for (uint32_t i = 0; i < n; i++) { const uint64_t e = offsets[i] + lens[i]; if (e > nbytes) nbytes = e; }
-  CK(ctx->d_bpe_text.ensure(nbytes + 64));
-  CK(ctx->d_bpe_off.ensure((size_t)n * 8));
-  CK(ctx->d_bpe_len.ensure((size_t)n * 4));
-  CK(ctx->d_bpe_cnt.ensure((size_t)n * 4));
-  cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->d_bpe_text, text, nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_bpe_off, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_bpe_len, lens, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  float ms = 0;
-  if (int rc = aigw_bpe_count_device(ctx, bpe, ctx->d_bpe_text, ctx->d_bpe_off, ctx->d_bpe_len, n, ctx->d_bpe_cnt, st, &ms)) return rc;
-  CK(cudaMemcpyAsync(counts, ctx->d_bpe_cnt, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (kernel_ms) *kernel_ms = ms;
-  if (h2d_bytes) *h2d_bytes = nbytes + (uint64_t)n * 12;
-  if (d2h_bytes) *d2h_bytes = (uint64_t)n * 4;
-  return 0;
+  HostStage S(ctx);
+  const uint8_t* d_text = S.span(text, offsets, lens, n);
+  const uint64_t* d_off = S.in(offsets, n);
+  const uint32_t* d_len = S.in(lens, n);
+  uint32_t* d_counts = S.out<uint32_t>(n);
+  if (S.rc) return S.rc;
+  if (int rc = aigw_bpe_count_device(ctx, bpe, d_text, d_off, d_len, n, d_counts, S.st, kernel_ms)) return rc;
+  S.back(counts, d_counts, n);
+  return S.wait(h2d_bytes, d2h_bytes);
 }
 
 // ------------------------------------------------------------------ large /v1/embeddings requests: ParseBody + BPE count (BASELINE config 3)
@@ -666,22 +772,19 @@ int aigw_embeddings_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t
   if (!ctx || !bpe) return -2;
   if (n == 0) return 0;
   ENTER();
-  uint64_t nbytes = 0; uint32_t max_len = 0;
-  for (uint32_t i = 0; i < n; i++) { const uint64_t e = offsets[i] + lens[i]; if (e > nbytes) nbytes = e; if (lens[i] > max_len) max_len = lens[i]; if (offsets[i] & 15u) { ctx->err = "aigw_embeddings_count_host: request starts must be 16-byte aligned"; return -2; } }
-  CK(ctx->d_emb_body.ensure(nbytes + 64));
-  CK(ctx->d_emb_off.ensure((size_t)n * 8));
-  CK(ctx->d_emb_len.ensure((size_t)n * 4));
-  CK(ctx->d_emb_res.ensure((size_t)n * sizeof(aigw_emb_count_result)));
-  cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->d_emb_body, bodies, nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_emb_off, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->d_emb_len, lens, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  if (int rc = aigw_embeddings_count_device(ctx, bpe, ctx->d_emb_body, ctx->d_emb_off, ctx->d_emb_len, n, max_len, nbytes, ctx->d_emb_res, st, kernel_ms)) return rc;
-  CK(cudaMemcpyAsync(results, ctx->d_emb_res, (size_t)n * sizeof(aigw_emb_count_result), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (h2d_bytes) *h2d_bytes = nbytes + (uint64_t)n * 12;
-  if (d2h_bytes) *d2h_bytes = (uint64_t)n * sizeof(aigw_emb_count_result) + 4;
-  return 0;
+  uint32_t max_len = 0;
+  for (uint32_t i = 0; i < n; i++) { if (lens[i] > max_len) max_len = lens[i]; if (offsets[i] & 15u) { ctx->err = "aigw_embeddings_count_host: request starts must be 16-byte aligned"; return -2; } }
+  HostStage S(ctx);
+  uint64_t nbytes = 0;
+  const uint8_t* d_bodies = S.span(bodies, offsets, lens, n, &nbytes);
+  const uint64_t* d_off = S.in(offsets, n);
+  const uint32_t* d_len = S.in(lens, n);
+  aigw_emb_count_result* d_res = S.out<aigw_emb_count_result>(n);
+  if (S.rc) return S.rc;
+  if (int rc = aigw_embeddings_count_device(ctx, bpe, d_bodies, d_off, d_len, n, max_len, nbytes, d_res, S.st, kernel_ms)) return rc;
+  S.back(results, d_res, n);
+  S.d2h += 4;   // the device form's read-back of the text count
+  return S.wait(h2d_bytes, d2h_bytes);
 }
 
 // ------------------------------------------------------------------ SSE
@@ -698,26 +801,15 @@ int aigw_sse_usage_host(aigw_ctx* ctx, const uint8_t* bytes, const uint64_t* chu
                         uint32_t n_streams, uint32_t n_chunks, aigw_sse_result* results, uint64_t* h2d_bytes, uint64_t* d2h_bytes, float* kernel_ms) {
   if (n_streams == 0) return 0;
   ENTER();
-  const uint64_t nbytes = chunk_off[n_chunks];
-  CK(ctx->stage_bytes.ensure(nbytes + 64));
-  CK(ctx->stage_off.ensure(((size_t)n_chunks + 1) * 8));
-  CK(ctx->stage_len.ensure(((size_t)n_streams + 1) * 4));
-  CK(ctx->stage_res.ensure((size_t)n_streams * sizeof(aigw_sse_result)));
-  cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->stage_bytes, bytes, nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->stage_off, chunk_off, ((size_t)n_chunks + 1) * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->stage_len, chunk_first, ((size_t)n_streams + 1) * 4, cudaMemcpyHostToDevice, st));
-  SseParams P; P.bytes = ctx->stage_bytes; P.chunk_off = ctx->stage_off; P.chunk_first = ctx->stage_len; P.n_streams = n_streams; P.results = ctx->stage_res;
-  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
-  CK(cudaEventRecord(ctx->ev0, st));
-  CK(launch_sse_usage(P, ctx->sm_count, st));
-  CK(cudaEventRecord(ctx->ev1, st));
-  CK(cudaMemcpyAsync(results, ctx->stage_res, (size_t)n_streams * sizeof(aigw_sse_result), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, ctx->ev0, ctx->ev1));
-  if (h2d_bytes) *h2d_bytes = nbytes + ((uint64_t)n_chunks + 1) * 8 + ((uint64_t)n_streams + 1) * 4;
-  if (d2h_bytes) *d2h_bytes = (uint64_t)n_streams * sizeof(aigw_sse_result);
-  return 0;
+  HostStage S(ctx);
+  const uint8_t* d_bytes = S.in(bytes, chunk_off[n_chunks]);
+  const uint64_t* d_chunk_off = S.in(chunk_off, (size_t)n_chunks + 1);
+  const uint32_t* d_chunk_first = S.in(chunk_first, (size_t)n_streams + 1);
+  aigw_sse_result* d_res = S.out<aigw_sse_result>(n_streams);
+  if (S.rc) return S.rc;
+  if (int rc = aigw_sse_usage_device(ctx, d_bytes, d_chunk_off, d_chunk_first, n_streams, d_res, S.st, kernel_ms)) return rc;
+  S.back(results, d_res, n_streams);
+  return S.wait(h2d_bytes, d2h_bytes);
 }
 
 // ------------------------------------------------------------------ stateful per-chunk response streams
@@ -896,6 +988,12 @@ static int fill_stream_params(aigw_ctx* ctx, BedrockStreamParams& P, const aigw_
   P.id_len = (uint32_t)strlen(id); memcpy(P.id, id, P.id_len); P.model_len = (uint32_t)strlen(model); memcpy(P.model, model, P.model_len);
   return 0;
 }
+// one batch of streams on st, P's buffers set and d_bs_work large enough: the device form, and each chunk of the host form
+static int bedrock_stream_device_impl(aigw_ctx* ctx, BedrockStreamParams& P, cudaStream_t st, float* kernel_ms) {
+  bedrock_work_layout(P, ctx->d_bs_work, P.n_streams);
+  if (int rc = take_counters(ctx, 2, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_bedrock_stream(P, ctx->sm_count, st)); return 0; });
+}
 int aigw_bedrock_stream_device(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, const uint8_t* d_bytes, const uint64_t* d_stream_off, uint32_t n_streams,
                                uint64_t total_bytes, uint8_t* d_out, uint64_t out_capacity, aigw_stream_result* d_results, uint64_t* d_out_used,
                                void* stream, float* kernel_ms) {
@@ -907,11 +1005,10 @@ int aigw_bedrock_stream_device(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg
   CK(ctx->d_bs_work.ensure(bedrock_work_bytes(total_bytes, n_streams)));
   P.bytes = d_bytes; P.stream_off = d_stream_off; P.off_base = 0; P.out_bias = 0; P.n_streams = n_streams; P.out = d_out; P.out_capacity = out_capacity; P.results = d_results;
   P.out_used = (unsigned long long*)d_out_used;
-  bedrock_work_layout(P, ctx->d_bs_work, n_streams);
-  if (int rc = take_counters(ctx, 2, st, &P.next)) return rc;
   CK(cudaMemsetAsync(d_out_used, 0, sizeof(uint64_t), st));
-  return timed(ctx, st, kernel_ms, [&] { CK(launch_bedrock_stream(P, ctx->sm_count, st)); return 0; });
+  return bedrock_stream_device_impl(ctx, P, st, kernel_ms);
 }
+
 int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, const uint8_t* bytes, const uint64_t* stream_off, uint32_t n_streams,
                              uint64_t out_capacity_hint, aigw_stream_batch_out* out) {
   memset(out, 0, sizeof *out);
@@ -919,64 +1016,19 @@ int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, 
   ENTER();
   BedrockStreamParams P0;
   if (int rc = fill_stream_params(ctx, P0, cfg)) return rc;
-  // sub-batches of ~64 MiB of stream bytes
-  constexpr uint64_t kChunk = 64ull << 20;
-  const std::vector<uint32_t> cb = chunk_bounds(n_streams, kChunk, [&](uint32_t i) { return stream_off[i]; }, [&](uint32_t i) { return stream_off[i + 1]; });
-  const int nch = (int)cb.size() - 1;
   const uint64_t total_in = stream_off[n_streams] - stream_off[0];
   const double ratio = out_capacity_hint ? (double)out_capacity_hint / (double)(total_in + 1) : 2.0;
-  std::vector<uint64_t> out_cap(nch), out_base(nch);
-  uint64_t max_in = 0, total_cap = 0; uint32_t max_n = 0;
-  for (int c = 0; c < nch; c++) {
-    const uint64_t ib = stream_off[cb[c + 1]] - stream_off[cb[c]]; const uint32_t nd = cb[c + 1] - cb[c];
-    if (ib > max_in) max_in = ib; if (nd > max_n) max_n = nd;
-    out_cap[c] = ((uint64_t)((double)ib * ratio) + (uint64_t)nd * 64 + 4096 + 255) & ~255ull;
-    out_base[c] = total_cap; total_cap += out_cap[c];
-  }
-  const int nslots = nch < 2 ? 1 : 2;
-  for (int k = 0; k < nslots; k++) {
-    CK(ctx->slot[k].d_in.ensure(max_in + 64));
-    CK(ctx->d_bs_off[k].ensure(((size_t)max_n + 1) * 8));
-  }
-  CK(ctx->d_bs_work.ensure(bedrock_work_bytes(max_in, max_n)));
-  CK(ctx->h_out.ensure(total_cap));
-  CK(ctx->h_sres.ensure((size_t)n_streams * sizeof(aigw_stream_result)));
-  CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
-  uint8_t* dev_out = nullptr; aigw_stream_result* dev_res = nullptr;
-  CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0));
-  CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_sres, 0));
-  uint64_t h2d = 0;
-  CK(cudaMemsetAsync(ctx->d_used_arr, 0, (size_t)nch * 8, ctx->s_compute));
-  CK(cudaEventRecord(ctx->ev0, ctx->s_compute));
-  for (int c = 0; c < nch; c++) {
-    ChunkSlot& S = ctx->slot[c % nslots];
-    uint64_t* d_off = ctx->d_bs_off[c % nslots];
-    const uint32_t b = cb[c], e = cb[c + 1], nd = e - b;
-    const uint64_t ib = stream_off[e] - stream_off[b];
-    if (c >= nslots) CK(cudaStreamWaitEvent(ctx->s_h2d, S.ev_k1, 0));
-    CK(cudaMemcpyAsync(S.d_in, bytes + stream_off[b], ib, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(d_off, stream_off + b, ((size_t)nd + 1) * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaEventRecord(S.ev_h2d, ctx->s_h2d));
-    h2d += ib + ((uint64_t)nd + 1) * 8;
-    CK(cudaStreamWaitEvent(ctx->s_compute, S.ev_h2d, 0));
-    BedrockStreamParams P = P0;
-    P.bytes = S.d_in - stream_off[b]; P.stream_off = d_off; P.off_base = stream_off[b]; P.n_streams = nd;
-    P.out = dev_out + out_base[c]; P.out_capacity = out_cap[c]; P.out_bias = out_base[c];
-    P.results = dev_res + b; P.out_used = ctx->d_used_arr + c;
-    bedrock_work_layout(P, ctx->d_bs_work, nd);
-    if (int rc = take_counters(ctx, 2, ctx->s_compute, &P.next)) return rc;
-    CK(launch_bedrock_stream(P, ctx->sm_count, ctx->s_compute));
-    CK(cudaEventRecord(S.ev_k1, ctx->s_compute));
-    out->gpu_launches += 2;
-  }
-  CK(cudaEventRecord(ctx->ev1, ctx->s_compute));
-  CK(cudaMemcpyAsync(ctx->h_used_arr, ctx->d_used_arr, (size_t)nch * 8, cudaMemcpyDeviceToHost, ctx->s_compute));
-  CK(cudaStreamSynchronize(ctx->s_compute));
-  uint64_t d2h = (uint64_t)n_streams * sizeof(aigw_stream_result) + (uint64_t)nch * 8;
-  for (int c = 0; c < nch; c++) d2h += ctx->h_used_arr[c] < out_cap[c] ? ctx->h_used_arr[c] : out_cap[c];
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  out->results = ctx->h_sres; out->out = ctx->h_out; out->out_used = total_cap; out->h2d_bytes = h2d; out->d2h_bytes = d2h; out->kernel_ms = ms;
-  return 0;
+  return chunk_pipeline(
+      ctx, bytes, stream_off, nullptr, n_streams, 64ull << 20,
+      [&](uint64_t ib, uint32_t nd) { return ((uint64_t)((double)ib * ratio) + (uint64_t)nd * 64 + 4096 + 255) & ~255ull; }, 2,
+      [&](const PipeChunk<aigw_stream_result>& k) {
+        CK(ctx->d_bs_work.ensure(bedrock_work_bytes(k.max_in, k.max_n)));   // the chunks share it: sized once, by the first
+        BedrockStreamParams P = P0;
+        P.bytes = k.bytes; P.stream_off = k.off; P.off_base = stream_off[k.first]; P.n_streams = k.n;
+        P.out = k.out; P.out_capacity = k.out_cap; P.out_bias = k.out_bias; P.results = k.results; P.out_used = k.out_used;
+        return bedrock_stream_device_impl(ctx, P, ctx->s_compute, nullptr);
+      },
+      out);
 }
 
 // ------------------------------------------------------------------ B1: body mutation
@@ -1054,6 +1106,11 @@ static int fill_mutate_params(aigw_ctx* ctx, MutateParams& P, const aigw_body_mu
   P.n_keys = (uint32_t)keys.size();
   return 0;
 }
+// one batch of bodies on st, P's buffers set: the device form, and each chunk of the host form
+static int body_mutate_device_impl(aigw_ctx* ctx, MutateParams& P, uint32_t max_len, cudaStream_t st, float* kernel_ms) {
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_body_mutate(P, max_len, ctx->sm_count, st)); return 0; });
+}
 int aigw_body_mutate_device(aigw_ctx* ctx, const aigw_body_mutation* m, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
                             uint32_t max_len, uint8_t* d_out, uint64_t out_capacity, aigw_mut_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
   if (kernel_ms) *kernel_ms = 0;
@@ -1063,14 +1120,11 @@ int aigw_body_mutate_device(aigw_ctx* ctx, const aigw_body_mutation* m, const ui
   if (int rc = fill_mutate_params(ctx, P, m)) return rc;
   P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.out = d_out; P.out_capacity = out_capacity; P.out_bias = 0; P.results = d_results;
   P.out_used = (unsigned long long*)d_out_used;
-  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
   CK(cudaMemsetAsync(d_out_used, 0, sizeof(uint64_t), st));
-  return timed(ctx, st, kernel_ms, [&] { CK(launch_body_mutate(P, max_len ? max_len : 65536u, ctx->sm_count, st)); return 0; });
+  return body_mutate_device_impl(ctx, P, max_len ? max_len : 65536u, st, kernel_ms);
 }
 int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
                           aigw_mut_batch_out* out) {
-  // Same pipeline as aigw_chat_translate_host: 256 MiB chunks, the H2D copy of chunk c+1 overlaps the kernel of chunk c, the
-  // kernel stores records and results straight into mapped pinned host memory, one synchronisation at the end.
   memset(out, 0, sizeof *out);
   if (n == 0) return 0;
   ENTER();
@@ -1078,62 +1132,18 @@ int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint
   if (int rc = fill_mutate_params(ctx, P0, m)) return rc;
   uint64_t extra = 0;
   for (uint32_t k = 0; k < P0.n_keys; k++) extra += P0.keys[k].memb_len + 2;
-  const uint64_t kChunkBytes = 256ull << 20;
-  const std::vector<uint32_t> cb = chunk_bounds(n, kChunkBytes, [&](uint32_t i) { return offsets[i]; }, [&](uint32_t i) { return offsets[i] + lens[i]; });
   uint32_t max_len = 0;
   for (uint32_t i = 0; i < n; i++) if (lens[i] > max_len) max_len = lens[i];
-  const int nch = (int)cb.size() - 1;
-  std::vector<uint64_t> in_bytes(nch), out_cap(nch), out_base(nch);
-  uint64_t max_in = 0, total_cap = 0; uint32_t max_docs = 0;
-  for (int c = 0; c < nch; c++) {
-    const uint32_t b = cb[c], e = cb[c + 1];
-    const uint64_t ib = offsets[e - 1] + lens[e - 1] - offsets[b];
-    in_bytes[c] = ib; if (ib > max_in) max_in = ib; if (e - b > max_docs) max_docs = e - b;
-    out_cap[c] = (ib + (uint64_t)(e - b) * (extra + 32) + 4096 + 255) & ~255ull;
-    out_base[c] = total_cap; total_cap += out_cap[c];
-  }
-  const int nslots = nch < 2 ? 1 : 2;
-  for (int k = 0; k < nslots; k++) {
-    ChunkSlot& S = ctx->slot[k];
-    CK(S.d_in.ensure(max_in + 64));
-    CK(S.d_off.ensure((size_t)max_docs * 8)); CK(S.d_len.ensure((size_t)max_docs * 4));
-  }
-  CK(ctx->h_out.ensure(total_cap));
-  CK(ctx->h_mres.ensure((size_t)n * sizeof(aigw_mut_result)));
-  CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
-  uint8_t* dev_out = nullptr; aigw_mut_result* dev_res = nullptr;
-  CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0));
-  CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_mres, 0));
-  uint64_t h2d = 0;
-  CK(cudaMemsetAsync(ctx->d_used_arr, 0, (size_t)nch * 8, ctx->s_compute));
-  CK(cudaEventRecord(ctx->ev0, ctx->s_compute));
-  for (int c = 0; c < nch; c++) {
-    ChunkSlot& S = ctx->slot[c % nslots];
-    const uint32_t b = cb[c], e = cb[c + 1], nd = e - b;
-    if (c >= nslots) CK(cudaStreamWaitEvent(ctx->s_h2d, S.ev_k1, 0));
-    CK(cudaMemcpyAsync(S.d_in, bodies + offsets[b], in_bytes[c], cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(S.d_off, offsets + b, (size_t)nd * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(S.d_len, lens + b, (size_t)nd * 4, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaEventRecord(S.ev_h2d, ctx->s_h2d));
-    h2d += in_bytes[c] + (uint64_t)nd * 12;
-    CK(cudaStreamWaitEvent(ctx->s_compute, S.ev_h2d, 0));
-    MutateParams P = P0;
-    P.bodies = S.d_in - offsets[b]; P.offsets = S.d_off; P.lens = S.d_len; P.n = nd;
-    P.out = dev_out + out_base[c]; P.out_capacity = out_cap[c]; P.out_bias = out_base[c]; P.results = dev_res + b;
-    P.out_used = ctx->d_used_arr + c;
-    if (int rc = take_counters(ctx, 1, ctx->s_compute, &P.next)) return rc;
-    CK(launch_body_mutate(P, max_len, ctx->sm_count, ctx->s_compute));
-    CK(cudaEventRecord(S.ev_k1, ctx->s_compute));
-    out->gpu_launches += 1;
-  }
-  CK(cudaEventRecord(ctx->ev1, ctx->s_compute));
-  CK(cudaMemcpyAsync(ctx->h_used_arr, ctx->d_used_arr, (size_t)nch * 8, cudaMemcpyDeviceToHost, ctx->s_compute));
-  CK(cudaStreamSynchronize(ctx->s_compute));
-  uint64_t d2h = (uint64_t)n * sizeof(aigw_mut_result) + (uint64_t)nch * 8;
-  for (int c = 0; c < nch; c++) d2h += ctx->h_used_arr[c] < out_cap[c] ? ctx->h_used_arr[c] : out_cap[c];
-  float ms = 0; cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-  out->results = ctx->h_mres; out->out = ctx->h_out; out->out_used = total_cap; out->h2d_bytes = h2d; out->d2h_bytes = d2h; out->kernel_ms = ms;
-  return 0;
+  return chunk_pipeline(
+      ctx, bodies, offsets, lens, n, 256ull << 20,
+      [&](uint64_t ib, uint32_t nd) { return (ib + (uint64_t)nd * (extra + 32) + 4096 + 255) & ~255ull; }, 1,
+      [&](const PipeChunk<aigw_mut_result>& k) {
+        MutateParams P = P0;
+        P.bodies = k.bytes; P.offsets = k.off; P.lens = k.len; P.n = k.n;
+        P.out = k.out; P.out_capacity = k.out_cap; P.out_bias = k.out_bias; P.results = k.results; P.out_used = k.out_used;
+        return body_mutate_device_impl(ctx, P, max_len, ctx->s_compute, nullptr);
+      },
+      out);
 }
 
 // ------------------------------------------------------------------ SigV4 payload hash
@@ -1152,21 +1162,15 @@ int aigw_chat_body_sha256_device(aigw_ctx* ctx, const uint8_t* d_out, const aigw
 int aigw_sha256_host(aigw_ctx* ctx, const uint8_t* bytes, const uint64_t* off, const uint32_t* len, uint32_t n, uint8_t* digests) {
   if (n == 0) return 0;
   ENTER();
-  uint64_t lo = ~0ull, hi = 0;
-  for (uint32_t i = 0; i < n; i++) { if (off[i] < lo) lo = off[i]; if (off[i] + len[i] > hi) hi = off[i] + len[i]; }
-  const uint64_t nbytes = hi - lo;
-  ChunkSlot& S = ctx->slot[0];
-  CK(S.d_in.ensure(nbytes + 64));
-  CK(S.d_off.ensure((size_t)n * 8)); CK(S.d_len.ensure((size_t)n * 4));
-  CK(ctx->stage_res.ensure((size_t)n * 32));
-  cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(S.d_in, bytes + lo, nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(S.d_off, off, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(S.d_len, len, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  CK(launch_sha256(S.d_in - lo, S.d_off, S.d_len, nullptr, n, (uint8_t*)ctx->stage_res.p, st));
-  CK(cudaMemcpyAsync(digests, ctx->stage_res, (size_t)n * 32, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  HostStage S(ctx);
+  const uint8_t* d_bytes = S.span(bytes, off, len, n);
+  const uint64_t* d_off = S.in(off, n);
+  const uint32_t* d_len = S.in(len, n);
+  uint8_t* d_digests = S.out<uint8_t>((size_t)n * 32);
+  if (S.rc) return S.rc;
+  if (int rc = aigw_sha256_device(ctx, d_bytes, d_off, d_len, n, d_digests, S.st, nullptr)) return rc;
+  S.back(digests, d_digests, (size_t)n * 32);
+  return S.wait();
 }
 
 // ------------------------------------------------------------------ CEL cost expressions
@@ -1222,25 +1226,20 @@ int aigw_usage_costs_cel_host(aigw_ctx* ctx, const aigw_sse_result* results, uin
                               const char* backend, const char* route_name, uint64_t* costs, uint8_t* errs) {
   if (n == 0 || n_progs == 0) return 0;
   ENTER();
-  const size_t nres = (size_t)n * sizeof(aigw_sse_result), nout = (size_t)n * n_progs;
-  CK(ctx->stage_res.ensure(nres));
-  CK(ctx->stage_off.ensure(nout * 9 + 64));   // costs, then error codes
-  CK(ctx->stage_bytes.ensure(model_bytes_len + (size_t)n * 8 + 64));
-  cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->stage_res, results, nres, cudaMemcpyHostToDevice, st));
-  uint32_t* d_off = nullptr; uint32_t* d_len = nullptr;
-  if (model_off && model_len) {
-    d_off = (uint32_t*)ctx->stage_bytes.p; d_len = d_off + n;
-    uint8_t* d_mb = (uint8_t*)(d_len + n);
-    CK(cudaMemcpyAsync(d_off, model_off, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_len, model_len, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_mb, model_bytes, model_bytes_len, cudaMemcpyHostToDevice, st));
-    if (int rc = aigw_usage_costs_cel_device(ctx, ctx->stage_res, n, progs, n_progs, d_mb, d_off, d_len, model, backend, route_name, ctx->stage_off, (uint8_t*)ctx->stage_off.p + nout * 8, st)) return rc;
-  } else if (int rc = aigw_usage_costs_cel_device(ctx, ctx->stage_res, n, progs, n_progs, nullptr, nullptr, nullptr, model, backend, route_name, ctx->stage_off, (uint8_t*)ctx->stage_off.p + nout * 8, st)) return rc;
-  CK(cudaMemcpyAsync(costs, ctx->stage_off, nout * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(errs, (uint8_t*)ctx->stage_off.p + nout * 8, nout, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  const size_t nout = (size_t)n * n_progs;
+  const bool spans = model_off && model_len;   // a request model per record
+  HostStage S(ctx);
+  const aigw_sse_result* d_results = S.in(results, n);
+  const uint32_t* d_model_off = spans ? S.in(model_off, n) : nullptr;
+  const uint32_t* d_model_len = spans ? S.in(model_len, n) : nullptr;
+  const uint8_t* d_model_bytes = spans ? S.in(model_bytes, model_bytes_len) : nullptr;
+  uint64_t* d_costs = S.out<uint64_t>(nout);
+  uint8_t* d_errs = S.out<uint8_t>(nout);
+  if (S.rc) return S.rc;
+  if (int rc = aigw_usage_costs_cel_device(ctx, d_results, n, progs, n_progs, d_model_bytes, d_model_off, d_model_len, model, backend, route_name, d_costs, d_errs, S.st)) return rc;
+  S.back(costs, d_costs, nout);
+  S.back(errs, d_errs, nout);
+  return S.wait();
 }
 
 // ------------------------------------------------------------------ R1 + C2
@@ -1271,26 +1270,22 @@ static int response_usage_host_impl(aigw_ctx* ctx, const uint8_t* bodies, const 
                                     const int32_t* cost_types, uint32_t n_costs, uint64_t* costs, int embeddings) {
   if (n == 0) return 0;
   ENTER();
-  const uint64_t nbytes = offsets[n - 1] + lens[n - 1] - offsets[0];
-  CK(ctx->stage_bytes.ensure(nbytes + 64));
-  CK(ctx->stage_off.ensure(((size_t)n + 1) * 8 + (size_t)n_costs * 8 * n + 64));   // offsets, then costs
-  CK(ctx->stage_len.ensure(((size_t)n + 1) * 4 + (size_t)n_costs * 4 + 64));        // lengths, then cost types
-  CK(ctx->stage_res.ensure((size_t)n * sizeof(aigw_sse_result)));
-  cudaStream_t st = ctx->s_compute;
-  CK(cudaMemcpyAsync(ctx->stage_bytes, bodies + offsets[0], nbytes, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->stage_off, offsets, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(ctx->stage_len, lens, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  CK(launch_response_usage(ctx->stage_bytes - offsets[0], ctx->stage_off, ctx->stage_len, n, ctx->stage_res, st, embeddings));
-  CK(cudaMemcpyAsync(results, ctx->stage_res, (size_t)n * sizeof(aigw_sse_result), cudaMemcpyDeviceToHost, st));
+  HostStage S(ctx);
+  const uint8_t* d_bodies = S.span(bodies, offsets, lens, n);
+  const uint64_t* d_offsets = S.in(offsets, n);
+  const uint32_t* d_lens = S.in(lens, n);
+  aigw_sse_result* d_results = S.out<aigw_sse_result>(n);
+  if (S.rc) return S.rc;
+  if (int rc = response_usage_device_impl(ctx, d_bodies, d_offsets, d_lens, n, d_results, S.st, nullptr, embeddings)) return rc;   // untimed: no wait
+  S.back(results, d_results, n);
   if (n_costs && costs) {
-    int32_t* d_types = (int32_t*)(ctx->stage_len + n + 1);
-    unsigned long long* d_costs = (unsigned long long*)(ctx->stage_off + n + 1);
-    CK(cudaMemcpyAsync(d_types, cost_types, (size_t)n_costs * 4, cudaMemcpyHostToDevice, st));
-    CK(launch_usage_costs(ctx->stage_res, n, d_types, n_costs, d_costs, st));
-    CK(cudaMemcpyAsync(costs, d_costs, (size_t)n * n_costs * 8, cudaMemcpyDeviceToHost, st));
+    const int32_t* d_cost_types = S.in(cost_types, n_costs);
+    uint64_t* d_costs = S.out<uint64_t>((size_t)n * n_costs);
+    if (S.rc) return S.rc;
+    if (int rc = aigw_usage_costs_device(ctx, d_results, n, d_cost_types, n_costs, d_costs, S.st)) return rc;
+    S.back(costs, d_costs, (size_t)n * n_costs);
   }
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  return S.wait();
 }
 int aigw_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
                              const int32_t* cost_types, uint32_t n_costs, uint64_t* costs) {

@@ -168,7 +168,10 @@ typedef struct aigw_usage { uint32_t input, output, total, cached, cache_creatio
  * The *_device entry points take a caller stream but share the context's workspace, counters and timing events: at most ONE call
  * may be in flight per context (synchronise, or order the next call after the previous one on the same stream).
  * aigw_batcher_* is the one entry point meant to be called concurrently (its launches use no context state); aigw_stream_* calls
- * serialise on a per-context mutex. */
+ * serialise on a per-context mutex.
+ * The single-shot host-buffer forms (aigw_bpe_count_host, aigw_embeddings_count_host, aigw_sse_usage_host, aigw_sha256_host,
+ * aigw_usage_costs_cel_host, aigw_*response_usage_host) copy their inputs in, run their *_device form and copy the outputs back
+ * before they return.  Their (bytes, offsets, lens) tables may list the bodies in any order. */
 int  aigw_init(int device, aigw_ctx** ctx);          /* returns 0, or a CUDA error code; never falls back */
 void aigw_destroy(aigw_ctx* ctx);
 const char* aigw_last_error(aigw_ctx* ctx);
@@ -404,6 +407,8 @@ typedef struct aigw_mut_result { uint64_t out_off; uint32_t out_len; uint8_t sta
 typedef struct aigw_mut_batch_out { const aigw_mut_result* results; const uint8_t* out; uint64_t out_used; uint64_t h2d_bytes, d2h_bytes; uint32_t gpu_launches; float kernel_ms; } aigw_mut_batch_out;
 int aigw_body_mutate_device(aigw_ctx* ctx, const aigw_body_mutation* m, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
                             uint32_t max_len, uint8_t* d_out, uint64_t out_capacity, aigw_mut_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+/* Host-buffer form: the bodies must lie in arena order (offsets ascending), since the call copies chunks of consecutive bodies, each
+ * as one span.  Pipelined like aigw_bedrock_stream_host; the views in `out` stay valid until the next host call on this ctx. */
 int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
                           aigw_mut_batch_out* out);
 

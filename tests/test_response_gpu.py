@@ -87,6 +87,25 @@ def test_response_usage_parity(ctx):
     assert n_ok > 2400
 
 
+def test_response_usage_host_any_offset_order(ctx):
+    """the host form stages every body whatever the order of the offset table: with the last two rows of the offset and length
+    tables swapped, each record equals the record of the same body in arena order"""
+    import aigw_b200 as A
+    bodies = [json.dumps({"id": "chatcmpl-%d" % i, "object": "chat.completion", "model": "gpt-4o-mini",
+                          "choices": [{"index": 0, "message": {"role": "assistant", "content": "ok " * (i % 9)}, "finish_reason": "stop"}],
+                          "usage": {"prompt_tokens": i, "completion_tokens": 2 * i, "total_tokens": 3 * i}}, separators=(",", ":")).encode() for i in range(300)]
+    arena, offs, lens = A.pack_bodies(bodies)
+    n = len(bodies)
+    perm = np.arange(n)
+    perm[[n - 2, n - 1]] = perm[[n - 1, n - 2]]
+    # the swapped call runs first, so that no earlier call of this test has staged the last body's bytes
+    swapped, swapped_costs = ctx.response_usage_host(arena, offs[:n][perm].copy(), lens[perm].copy(), cost_types=(0, 3, 4))
+    ordered, costs = ctx.response_usage_host(arena, offs, lens, cost_types=(0, 3, 4))
+    assert (ordered["status"] == 0).all() and int(ordered[n - 1]["input"]) == n - 1
+    assert ordered[perm].tobytes() == swapped.tobytes()
+    assert np.array_equal(costs[perm], swapped_costs)
+
+
 def test_reference_response_golden(ctx):
     """testupstream_test.go:266: OpenAI passthrough response without usage: counters set to zero, no model."""
     import aigw_b200 as A

@@ -71,8 +71,8 @@ def test_translate_record_bodies(gw):
 
 
 def test_translate_host_after_larger_hash_host():
-    """the hash and translate host calls stage offsets and lengths in the same chunk slot: a translate call after a larger hash call
-    on a fresh context still gets a result table for its own batch"""
+    """a larger hash host call leaves the translate pipeline's chunk slots alone: a translate call after it on a fresh context still
+    gets a result table for its own batch"""
     from aigw_b200 import capi
     c = capi.Context(0)
     try:
