@@ -10,8 +10,9 @@
 // characters in BASELINE config 3 — would leave most lanes idle one text at a time), stages the bytes, turns
 // them into symbol ids, finds the piece starts with ballots, and then every LANE runs the merge loop of one piece at a time
 // (pieces are independent).  Per piece the ranks of the adjacent pairs are kept next to the symbols, so a merge costs two
-// table lookups and one shift instead of a rescan.  A text longer than the buffer is cut at piece boundaries; a single piece
-// longer than the buffer is DECLINED (count 0xFFFFFFFF) rather than approximated.  sm_90a only.
+// table lookups and one shift instead of a rescan.  A text longer than the buffer is cut at piece boundaries; a text with a
+// piece longer than the buffer (512 bytes, its leading space included) is DECLINED (count 0xFFFFFFFF) rather than approximated.
+// sm_90a only.
 #include "bpe_kernel.cuh"
 
 #include <cstdio>
@@ -79,8 +80,11 @@ __global__ void __launch_bounds__(kBpeWarps * 32, 1) bpe_count_kernel(const BpeP
         uint32_t take = len;
         if (fill + len > (uint32_t)kBpeBuf) {
           if (nt > 0) break;                                   // what is staged so far is counted first
-          uint32_t cut = 0;                                    // the last piece start inside the window
+          // the last piece start in src[1 .. kBpeBuf]; src[kBpeBuf] is readable (len > kBpeBuf), and a start there means the window
+          // holds whole pieces, so a text is declined exactly when one of its pieces is longer than the buffer
+          uint32_t cut = 0;
           for (uint32_t b0 = 0; b0 < (uint32_t)kBpeBuf; b0 += 32) { const uint32_t i = b0 + lane; const uint32_t m = __ballot_sync(0xffffffffu, i > 0 && src[i] == ' '); if (m) cut = b0 + 31u - __clz(m); }
+          if (src[kBpeBuf] == ' ') cut = kBpeBuf;
           if (cut == 0) { if (lane == 0) P.counts[t] = 0xffffffffu; t++; t_off = 0; t_acc = 0; break; }   // one piece longer than the buffer: declined
           take = cut; last_partial = true;
         }

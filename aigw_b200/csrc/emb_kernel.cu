@@ -35,6 +35,7 @@ struct EmbShared {
   uint32_t doc; uint32_t fail;   // lowest reason code raised by any thread (declines, below 32, win over the definite errors); kNoFail = none
   uint32_t n_lc, n_rc, n_lb, n_rb, lb, rb;
   uint32_t text_base, n_inputs, str_open, str_close;
+  uint32_t n_blank;   // rows below the text table's capacity that a request straddling it was handed (written as empty texts)
 };
 
 // JSON scalar in [p, p+n): 0 invalid, 1 null, 2 true / false, 3 integer (-?digits, at most 18), 4 other number
@@ -69,7 +70,7 @@ __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanP
   uint32_t* tok = P.tok_ws + (size_t)blockIdx.x * P.tok_cap;
   for (;;) {
     __syncthreads();
-    if (tid == 0) { S.doc = atomicAdd(P.next, 1u); S.fail = kNoFail; S.n_lc = S.n_rc = S.n_lb = S.n_rb = 0; S.lb = 0xffffffffu; S.rb = 0; S.n_inputs = 0; S.text_base = 0; S.str_open = S.str_close = 0; }
+    if (tid == 0) { S.doc = atomicAdd(P.next, 1u); S.fail = kNoFail; S.n_lc = S.n_rc = S.n_lb = S.n_rb = 0; S.lb = 0xffffffffu; S.rb = 0; S.n_inputs = 0; S.text_base = 0; S.str_open = S.str_close = 0; S.n_blank = 0; }
     __syncthreads();
     const uint32_t doc = S.doc;
     if (doc >= P.n) break;
@@ -116,7 +117,9 @@ __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanP
       const uint32_t inside = ps & ~c.quote;
       const uint32_t out = ~ps & ~c.quote;
       if (c.ctl & inside) fail = AIGW_R_CTRL_IN_STRING;
-      if (c.ctl & out & ~c.ws) fail = AIGW_R_SYNTAX;
+      // a raw control byte outside a string is a definite syntax error (400), unless a decline of this thread (an escape can
+      // make the string parity wrong) or of another one (the CTA keeps the lowest reason) comes first
+      if ((c.ctl & out & ~c.ws) && !fail) fail = AIGW_R_E400_SYNTAX;
       const uint32_t sc = out & ~c.op & ~c.ws;
       if (lane == 31) S.wlast[it][warp] = sc >> 31;
       uint32_t prev = __shfl_up_sync(0xffffffffu, sc >> 31, 1);
@@ -225,7 +228,8 @@ __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanP
       if (!f && model_l > 0xffffu) f = AIGW_R_TOO_LARGE;
       if (!f && n_inputs) {
         const uint32_t b = atomicAdd(P.text_used, n_inputs);
-        if ((uint64_t)b + n_inputs > P.text_cap) f = AIGW_R_ARENA_FULL; else S.text_base = b;
+        if ((uint64_t)b + n_inputs > P.text_cap) { f = AIGW_R_ARENA_FULL; if (b < P.text_cap) { S.text_base = b; S.n_blank = P.text_cap - b; } }
+        else S.text_base = b;
       }
       if (f) S.fail = (uint32_t)f;
       else { res.model_off = model_o; res.model_len = (uint16_t)model_l; S.n_inputs = n_inputs; S.str_open = s_open; S.str_close = s_close; }
@@ -240,6 +244,11 @@ __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanP
           P.text_off[tb + k] = boff + o + 1u; P.text_len[tb + k] = cpos - o - 1u;
         }
       } else if (n == 1 && tid == 0) { P.text_off[tb] = boff + S.str_open + 1u; P.text_len[tb] = S.str_close - S.str_open - 1u; }
+    } else {
+      // a declined request that straddles the capacity still owns rows below it, and the count kernel reads every row below it:
+      // empty texts, so that no row of an earlier call is read
+      const uint32_t nb = S.n_blank, tb = S.text_base;
+      for (uint32_t k = tid; k < nb; k += kEmbThreads) { P.text_off[tb + k] = boff; P.text_len[tb + k] = 0; }
     }
     if (tid == 0) {
       const int f = S.fail == kNoFail ? 0 : (int)S.fail;

@@ -671,7 +671,9 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
 // ------------------------------------------------------------------ K4: BPE token count
 int aigw_bpe_load(aigw_ctx* ctx, const uint16_t* byte_to_id, const uint32_t* merges, uint32_t n_merges, aigw_bpe** out) {
   if (!ctx || !byte_to_id || (!merges && n_merges) || !out || n_merges >= 65535u) return -2;
-  for (uint32_t r = 0; r < n_merges * 3; r++) if (merges[r] >= 65536u) return -2;
+  // ids stop at 65534: the pair (65535, 65535) would have key 0xFFFFFFFF, the empty-slot marker of the table
+  for (uint32_t i = 0; i < 256; i++) if (byte_to_id[i] >= 65535u) return -2;
+  for (uint32_t r = 0; r < n_merges * 3; r++) if (merges[r] >= 65535u) return -2;
   ENTER();
   uint32_t slots = 1024; while (slots < n_merges * 2u) slots <<= 1;
   if (bpe_smem_bytes(slots) > 220u * 1024u) { ctx->err = "aigw_bpe_load: merge table does not fit shared memory"; return -2; }
@@ -752,7 +754,9 @@ int aigw_embeddings_count_device(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8
   unsigned int n_texts = 0;
   CK(cudaMemcpyAsync(&n_texts, c1, sizeof n_texts, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (n_texts > text_cap) n_texts = text_cap;   // requests past the capacity were declined; rows below it are all valid
+  // requests past the capacity were declined (AIGW_R_ARENA_FULL); every row below it was written in this call, the rows of a
+  // request that straddles it as empty texts
+  if (n_texts > text_cap) n_texts = text_cap;
   if (kernel_ms) CK(cudaEventRecord(ev[2], st));
   if (n_texts) {
     BpeParams P; P.text = d_bodies; P.offsets = ctx->d_emb_toff; P.lens = ctx->d_emb_tlen; P.n = n_texts; P.counts = ctx->d_emb_cnt; P.table = bpe->d_table; P.slots = bpe->slots; P.byte_to_id = bpe->d_b2i; P.next = c2;

@@ -419,8 +419,12 @@ int aigw_body_mutate_host(aigw_ctx* ctx, const aigw_body_mutation* m, const uint
  *   pre-tokenisation  every space (0x20) starts a new piece; a piece is its first byte plus the bytes up to the next space
  *   model             bytes map to byte_to_id[]; inside a piece the adjacent pair of lowest merge rank is merged (leftmost first
  *                     among equal ranks) until no adjacent pair is in the merge table; tokens(text) = sum of final piece lengths
- * merges: n_merges triples (a, b, merged) of token ids < 65536, rank = position; n_merges < 65535.  Texts are raw bytes (already
- * JSON-unescaped).  counts[i] = 0xFFFFFFFF for a text that holds a space-free run longer than 512 bytes (declined, not approximated). */
+ * merges: n_merges triples (a, b, merged) of token ids, rank = position; a repeated pair keeps its first rank.  Every id, in
+ * byte_to_id and in merges, must be below 65535 (the pair (65535, 65535) would collide with the table's empty marker): aigw_bpe_load
+ * returns -2 otherwise, and also when the table (2 slots per merge, at least 1024, a power of two) does not fit shared memory
+ * beside the staging buffers, i.e. above 4096 merges.  Texts are raw bytes (already JSON-unescaped).
+ * counts[i] = 0xFFFFFFFF (declined, not approximated) exactly when text i has a piece longer than 512 bytes, a piece's leading
+ * space included: a text is counted when every piece fits the 512-byte staging buffer, wherever the long pieces lie. */
 typedef struct aigw_bpe aigw_bpe;
 int  aigw_bpe_load(aigw_ctx* ctx, const uint16_t* byte_to_id /* 256 */, const uint32_t* merges, uint32_t n_merges, aigw_bpe** out);
 void aigw_bpe_free(aigw_ctx* ctx, aigw_bpe* bpe);
@@ -434,11 +438,17 @@ int  aigw_bpe_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t* text
  * (internal/apischema/openai/union.go:71-147: "input" a string or an array of strings; openai.go:316-375 for the other members),
  * then the K4 count of every input, read in place from the request bytes (no text copy).  Requests may be far above the 64 KiB
  * ceiling of aigw_chat_translate_* (1024 inputs of 64 characters are 68.7 KB); one CTA streams one request.
- * status AIGW_OK: model span, n_inputs, tokens = sum of the inputs' counts (declined_inputs of them hold a space-free run above
- * 512 bytes and are not in the sum).  AIGW_MALFORMED_400: what ParseBody rejects (syntax, model / encoding_format / user not a
- * string, dimensions not an integer, input a number or a boolean).  AIGW_DECLINED (stock path decides): any backslash in the
- * request, nested containers (object inputs, token-id arrays), null or non-string array elements, members other than
- * model / input / encoding_format / dimensions / user, requests of 16 MiB and above. */
+ * status AIGW_OK: model span, n_inputs, tokens = sum of the inputs' counts (declined_inputs of them have a piece longer than
+ * 512 bytes, as aigw_bpe_count_* declines them, and are not in the sum).  AIGW_MALFORMED_400: what ParseBody rejects (syntax,
+ * model / encoding_format / user not a string, dimensions not an integer, input a number or a boolean).  AIGW_DECLINED (stock
+ * path decides): any backslash in the request, nested containers (object inputs, token-id arrays), null or non-string array
+ * elements, members other than model / input / encoding_format / dimensions / user, requests of 16 MiB and above
+ * (AIGW_R_TOO_LARGE), and two capacities of the call:
+ *   tokens      a request with more than max_len / 2 + 64 scan tokens (structural bytes outside strings, both quotes of every
+ *               string, the first byte of every scalar) is AIGW_R_TOKENS; max_len is the call's (the host form: its longest request)
+ *   text table  the call has total_bytes / 4 + 1024 rows, one per input; requests take their rows in the order their CTAs reach
+ *               them, and one whose rows would pass the end is AIGW_R_ARENA_FULL (which one depends on that order).  Only rows
+ *               written in this call are ever counted. */
 typedef struct aigw_emb_count_result {
   uint8_t  status;          /* enum aigw_status */
   uint8_t  reason;          /* enum aigw_reason */
