@@ -166,6 +166,12 @@ static_assert(CPK_COUNT <= 32, "the walk keeps the seen members in one 32-bit ma
   X("user", CPK_user) X("best_of", CPK_best_of) X("logit_bias", CPK_logit_bias) X("stream_options", CPK_stream_options) \
   X("include_usage", CPK_include_usage) X("presence_penalty", CPK_presence_penalty) X("frequency_penalty", CPK_frequency_penalty)
 
+// Cohere /v2/rerank requests (P.schema & AIGW_SCHEMA_RERANK): the members of cohere.RerankV2Request
+// (internal/apischema/cohere/rerank_v2.go).  No value ids.
+enum RRKid : uint8_t { RRK_NONE = 0, RRK_model, RRK_query, RRK_documents, RRK_top_n, RRK_max_tokens_per_doc, RRK_COUNT };
+#define AIGW_RRKEYS(X) \
+  X("model", RRK_model) X("query", RRK_query) X("documents", RRK_documents) X("top_n", RRK_top_n) X("max_tokens_per_doc", RRK_max_tokens_per_doc)
+
 static constexpr int kKeySlots = 128, kValSlots = 32, kMaxIdLen = 28, kIdWords = 7;
 // slot = { seven little-endian words of the string zero-padded to 28 bytes, len | id << 8 }
 struct IdSlot { uint32_t w[kIdWords]; uint32_t meta; };
@@ -248,6 +254,15 @@ constexpr IdTables make_cp_id_tables() {
 }
 static_assert(id_max_probe(make_cp_id_tables().key, kKeySlots) <= 6, "completions id hash table needs more than 6 probes");
 static __device__ __constant__ IdTables c_ids_cp = make_cp_id_tables();
+constexpr IdTables make_rr_id_tables() {
+  IdTables t{};
+#define X(lit, idv) id_insert(t.key, kKeySlots, lit, idv);
+  AIGW_RRKEYS(X)
+#undef X
+  return t;
+}
+static_assert(id_max_probe(make_rr_id_tables().key, kKeySlots) <= 6, "rerank id hash table needs more than 6 probes");
+static __device__ __constant__ IdTables c_ids_rr = make_rr_id_tables();
 
 // id of a short string (1 ≤ n ≤ kMaxIdLen) held in shared memory, against the key or the value table (also in shared
 // memory).  Straight-line code: seven aligned word loads, funnel shifts, length mask, multiplicative hash, ≤ 4 probes.

@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(WARPS * 32) chat_index_kernel(const __grid_con
   IdTables* s_ids = (IdTables*)smem;
   uint64_t* s_bar = (uint64_t*)(smem + sizeof(IdTables));
   {
-    const uint32_t* src = (const uint32_t*)((P.schema & AIGW_SCHEMA_COMPLETIONS) ? &c_ids_cp : (P.schema & AIGW_SCHEMA_RESPONSES) ? &c_ids_rq : (P.schema & AIGW_SCHEMA_MESSAGES) ? &c_ids_msg : (P.schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK ? &c_ids_resp : &c_ids);
+    const uint32_t* src = (const uint32_t*)((P.schema & AIGW_SCHEMA_RERANK) ? &c_ids_rr : (P.schema & AIGW_SCHEMA_COMPLETIONS) ? &c_ids_cp : (P.schema & AIGW_SCHEMA_RESPONSES) ? &c_ids_rq : (P.schema & AIGW_SCHEMA_MESSAGES) ? &c_ids_msg : (P.schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK ? &c_ids_resp : &c_ids);
     for (uint32_t i = threadIdx.x; i < sizeof(IdTables) / 4; i += blockDim.x) ((uint32_t*)s_ids)[i] = src[i];
   }
   if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }

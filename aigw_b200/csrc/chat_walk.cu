@@ -6,10 +6,10 @@
 namespace aigw {
 
 #define AIGW_WALK_DECL(g) cudaError_t launch_chat_walk_g##g(const ChatParams&, uint32_t, uint32_t, uint8_t*, const WorkLayout&, cudaStream_t, int);
-AIGW_WALK_DECL(0) AIGW_WALK_DECL(1) AIGW_WALK_DECL(2) AIGW_WALK_DECL(3) AIGW_WALK_DECL(4) AIGW_WALK_DECL(5) AIGW_WALK_DECL(6) AIGW_WALK_DECL(7) AIGW_WALK_DECL(8) AIGW_WALK_DECL(9) AIGW_WALK_DECL(10) AIGW_WALK_DECL(11)
+AIGW_WALK_DECL(0) AIGW_WALK_DECL(1) AIGW_WALK_DECL(2) AIGW_WALK_DECL(3) AIGW_WALK_DECL(4) AIGW_WALK_DECL(5) AIGW_WALK_DECL(6) AIGW_WALK_DECL(7) AIGW_WALK_DECL(8) AIGW_WALK_DECL(9) AIGW_WALK_DECL(10) AIGW_WALK_DECL(11) AIGW_WALK_DECL(12)
 #undef AIGW_WALK_DECL
 #define AIGW_SMALL_DECL(g) cudaError_t launch_chat_small_g##g(const ChatParams&, uint32_t, uint32_t, const uint64_t*, cudaStream_t);
-AIGW_SMALL_DECL(0) AIGW_SMALL_DECL(1) AIGW_SMALL_DECL(2) AIGW_SMALL_DECL(3) AIGW_SMALL_DECL(4) AIGW_SMALL_DECL(5) AIGW_SMALL_DECL(6) AIGW_SMALL_DECL(7) AIGW_SMALL_DECL(8) AIGW_SMALL_DECL(9) AIGW_SMALL_DECL(10) AIGW_SMALL_DECL(11)
+AIGW_SMALL_DECL(0) AIGW_SMALL_DECL(1) AIGW_SMALL_DECL(2) AIGW_SMALL_DECL(3) AIGW_SMALL_DECL(4) AIGW_SMALL_DECL(5) AIGW_SMALL_DECL(6) AIGW_SMALL_DECL(7) AIGW_SMALL_DECL(8) AIGW_SMALL_DECL(9) AIGW_SMALL_DECL(10) AIGW_SMALL_DECL(11) AIGW_SMALL_DECL(12)
 #undef AIGW_SMALL_DECL
 
 // resident walk blocks per SM.  The launch bound keeps room for AIGW_WALK_BLOCKS (the register budget), but the walk is bound by
@@ -26,6 +26,7 @@ cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs,
   if (blocks_per_sm <= 0 || blocks_per_sm > AIGW_WALK_BLOCKS) blocks_per_sm = env_ctas > 0 && env_ctas <= AIGW_WALK_BLOCKS ? env_ctas : kWalkBlocksPerSm;
   sms *= blocks_per_sm;
   const uint32_t s = P.schema;
+  if (s & (uint32_t)AIGW_SCHEMA_RERANK) return launch_chat_walk_g12(P, doc0, ndocs, work, layout, st, sms);   // declines every base but Cohere
   if (s & (uint32_t)AIGW_SCHEMA_COMPLETIONS) return launch_chat_walk_g11(P, doc0, ndocs, work, layout, st, sms);   // declines every base but OpenAI
   if (s & (uint32_t)AIGW_SCHEMA_RESPONSES) return launch_chat_walk_g10(P, doc0, ndocs, work, layout, st, sms);   // declines every base but OpenAI
   if (s & (uint32_t)AIGW_SCHEMA_MESSAGES)   // the full re-maps (OpenAI / Bedrock targets) have their own kernel
@@ -45,6 +46,7 @@ cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs,
 // fused small-batch kernel (one CTA per document, bodies of at most 5120 bytes): chat_walk_impl.cuh
 cudaError_t launch_chat_small(const ChatParams& P, uint32_t doc0, uint32_t ndocs, const uint64_t* out_slot, cudaStream_t st) {
   const uint32_t s = P.schema;
+  if (s & (uint32_t)AIGW_SCHEMA_RERANK) return launch_chat_small_g12(P, doc0, ndocs, out_slot, st);
   if (s & (uint32_t)AIGW_SCHEMA_COMPLETIONS) return launch_chat_small_g11(P, doc0, ndocs, out_slot, st);
   if (s & (uint32_t)AIGW_SCHEMA_RESPONSES) return launch_chat_small_g10(P, doc0, ndocs, out_slot, st);
   if (s & (uint32_t)AIGW_SCHEMA_MESSAGES)

@@ -231,12 +231,29 @@ static void fill_params(ChatParams& P, const aigw_backend_cfg* cfg) {
     memcpy(P.override_model, cfg->model_name_override, n); P.override_len = (uint16_t)n;
   }
   // path.Join("/", prefix, "chat/completions") (openai_openai.go:30), "embeddings", "responses" (openai_responses.go:52),
-  // "completions" (openai_completions.go:26)
+  // "completions" (openai_completions.go:26); rerank below
   std::string pfx = (cfg && cfg->openai_prefix) ? cfg->openai_prefix : "v1";
   while (!pfx.empty() && pfx.front() == '/') pfx.erase(0, 1);
   while (!pfx.empty() && pfx.back() == '/') pfx.pop_back();
   const char* endpoint = !cfg ? "chat/completions" : (cfg->schema & AIGW_SCHEMA_COMPLETIONS) ? "completions" : (cfg->schema & AIGW_SCHEMA_RESPONSES) ? "responses" : (cfg->schema & AIGW_SCHEMA_EMBEDDINGS) ? "embeddings" : "chat/completions";
   std::string path = "/" + (pfx.empty() ? std::string() : pfx + "/") + endpoint;
+  if (cfg && (cfg->schema & AIGW_SCHEMA_RERANK)) {
+    // path.Join("/", version, "rerank") (cohere_rerank_v2.go:26): the cleaned path, whose "." and ".." segments and doubled slashes
+    // are resolved (".." at the root stays at the root).  A path longer than openai_path leaves prefix_len 0 and the walk declines.
+    const std::string v = cfg->api_version ? cfg->api_version : "";
+    std::vector<std::string> segs;
+    for (size_t b = 0; b <= v.size();) {
+      size_t e = v.find('/', b); if (e == std::string::npos) e = v.size();
+      const std::string s = v.substr(b, e - b);
+      if (s == "..") { if (!segs.empty()) segs.pop_back(); }
+      else if (!s.empty() && s != ".") segs.push_back(s);
+      b = e + 1;
+    }
+    path.clear();
+    for (const std::string& s : segs) path += "/" + s;
+    path += "/rerank";
+    if (path.size() > sizeof P.openai_path) path.clear();
+  }
   if (path.size() > sizeof P.openai_path) path.resize(sizeof P.openai_path);
   memcpy(P.openai_path, path.data(), path.size()); P.prefix_len = (uint16_t)path.size();
   P.created = 0; P.rid_len = 0; memset(P.response_id, 0, sizeof P.response_id);
@@ -1269,6 +1286,10 @@ int aigw_responses_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies,
                                            aigw_sse_result* d_results, void* stream, float* kernel_ms) {
   return response_usage_device_impl(ctx, d_bodies, d_offsets, d_lens, n, d_results, stream, kernel_ms, 3);
 }
+int aigw_rerank_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
+                                      aigw_sse_result* d_results, void* stream, float* kernel_ms) {
+  return response_usage_device_impl(ctx, d_bodies, d_offsets, d_lens, n, d_results, stream, kernel_ms, 4);
+}
 
 static int response_usage_host_impl(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
                                     const int32_t* cost_types, uint32_t n_costs, uint64_t* costs, int embeddings) {
@@ -1306,6 +1327,10 @@ int aigw_completions_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, c
 int aigw_responses_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
                                          const int32_t* cost_types, uint32_t n_costs, uint64_t* costs) {
   return response_usage_host_impl(ctx, bodies, offsets, lens, n, results, cost_types, n_costs, costs, 3);
+}
+int aigw_rerank_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results,
+                                    const int32_t* cost_types, uint32_t n_costs, uint64_t* costs) {
+  return response_usage_host_impl(ctx, bodies, offsets, lens, n, results, cost_types, n_costs, costs, 4);
 }
 
 int aigw_usage_costs_device(aigw_ctx* ctx, const aigw_sse_result* d_results, uint32_t n, const int32_t* d_cost_types, uint32_t n_costs, uint64_t* d_costs, void* stream) {

@@ -325,6 +325,30 @@ __global__ void __launch_bounds__(128) completions_response_kernel(const uint8_t
   results[d] = r;
 }
 
+// Buffered Cohere /v2/rerank (cohere_rerank_v2.go:73-108): json.NewDecoder semantics as for /v1/responses.  A non-null meta.tokens
+// sets total; input_tokens / output_tokens set input / output when non-null (uint32 of the float64); total is their uint32 sum.  No
+// response model: the reference reports the request model.  Its own kernel: inlined into completions_response_kernel, the exact
+// float conversion made that kernel spill.
+__device__ SchemaBlob g_rerank_resp_schema;
+__global__ void __launch_bounds__(128) rerank_response_kernel(const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results) {
+  const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
+  if (d >= n) return;
+  Capture cp; cp.int_set = 0; cp.obj_seen = 0; cp.span_set = 0; cp.span_esc = 0; cp.weird = 0; cp.big = 0;
+#pragma unroll
+  for (int k = 0; k < 8; k++) cp.ints[k] = 0;
+  const bool ok = walk<Capture, false, true>(bodies + offsets[d], (int)lens[d], g_rerank_resp_schema.nodes, g_rerank_resp_schema.fields, g_rerank_resp_schema.keys, Q_ROOT, cp, /*allow_trailing=*/true);
+  aigw_sse_result r; memset(&r, 0, sizeof r);
+  if (cp.weird) r.status = AIGW_DECLINED;
+  else if (!ok) r.status = AIGW_INTERNAL;  // "failed to unmarshal body"
+  else if (cp.obj_seen & (1u << C_OBJ_USAGE)) {
+    r.usage.mask = 4u;
+    if (cp.int_set & (1u << C_PROMPT)) { r.usage.input = cp.ints[C_PROMPT]; r.usage.mask |= 1u; }
+    if (cp.int_set & (1u << C_COMPLETION)) { r.usage.output = cp.ints[C_COMPLETION]; r.usage.mask |= 2u; }
+    r.usage.total = r.usage.input + r.usage.output;
+  }
+  results[d] = r;
+}
+
 // C2: evalCost's direct selectors over a table of usages (internal/extproc/processor_impl.go:707-756)
 __global__ void usage_costs_kernel(const aigw_sse_result* results, uint32_t n, const int32_t* cost_types, uint32_t n_costs, unsigned long long* out) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -342,11 +366,13 @@ cudaError_t launch_response_usage(const uint8_t* bodies, const uint64_t* offsets
       RespSchemaBlob b = build_resp_schema(); cudaError_t e = cudaMemcpyToSymbol(g_resp_schema, &b, sizeof b); if (e != cudaSuccess) return e;
       RespSchemaBlob b2 = build_emb_schema(); e = cudaMemcpyToSymbol(g_emb_schema, &b2, sizeof b2); if (e != cudaSuccess) return e;
       SchemaBlob b3 = build_completion_schema(); e = cudaMemcpyToSymbol(g_cmpl_resp_schema, &b3, sizeof b3); if (e != cudaSuccess) return e;
-      RspSchemaBlob b4 = build_responses_schema(); return cudaMemcpyToSymbol(g_rsp_resp_schema, &b4, sizeof b4);
+      RspSchemaBlob b4 = build_responses_schema(); e = cudaMemcpyToSymbol(g_rsp_resp_schema, &b4, sizeof b4); if (e != cudaSuccess) return e;
+      SchemaBlob b5 = build_rerank_schema(); return cudaMemcpyToSymbol(g_rerank_resp_schema, &b5, sizeof b5);
     });
     if (e0 != cudaSuccess) return e0;
   }
   if (n == 0) return cudaSuccess;
+  if (embeddings == 4) { rerank_response_kernel<<<(n + 127) / 128, 128, 0, st>>>(bodies, offsets, lens, n, results); return cudaGetLastError(); }
   if (embeddings >= 2) { completions_response_kernel<<<(n + 127) / 128, 128, 0, st>>>(bodies, offsets, lens, n, results, embeddings == 3); return cudaGetLastError(); }
   response_usage_kernel<<<(n + 127) / 128, 128, 0, st>>>(bodies, offsets, lens, n, results, embeddings);
   return cudaGetLastError();

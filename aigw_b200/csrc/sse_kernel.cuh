@@ -35,7 +35,7 @@ struct SseParams {
 };
 
 cudaError_t launch_sse_usage(const SseParams& P, int sm_count, cudaStream_t st);
-cudaError_t launch_response_usage(const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results, cudaStream_t st, int embeddings = 0 /* 0 chat completion, 1 embeddings, 2 legacy completions, 3 /v1/responses */);
+cudaError_t launch_response_usage(const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_sse_result* results, cudaStream_t st, int embeddings = 0 /* 0 chat completion, 1 embeddings, 2 legacy completions, 3 /v1/responses, 4 Cohere /v2/rerank */);
 cudaError_t launch_usage_costs(const aigw_sse_result* results, uint32_t n, const int32_t* cost_types, uint32_t n_costs, unsigned long long* out, cudaStream_t st);
 
 }  // namespace aigw

@@ -212,6 +212,41 @@ static inline RspSchemaBlob build_responses_schema() {
   return b;
 }
 
+// ------------------------------------------------------------------ schema: cohere.RerankV2Response (walked by walk<CAP, true>)
+// internal/apischema/cohere/rerank_v2.go.  Every float64 member is K_F64; meta.tokens' two counts are captured as uint32(float64).
+enum QN : uint8_t { Q_ANY = 0, Q_STR, Q_INT, Q_F64, Q_BOOL, Q_ROOT, Q_RESULTS, Q_RESULT, Q_META, Q_APIVER, Q_BILLED, Q_TOKENS, Q_STRS,
+                    Q_IN, Q_OUT, Q_COUNT };
+static const FieldDef kRerankFields[] = {
+  {Q_ROOT, "results", Q_RESULTS}, {Q_ROOT, "id", Q_STR}, {Q_ROOT, "meta", Q_META},
+  {Q_RESULT, "index", Q_INT}, {Q_RESULT, "relevance_score", Q_F64},
+  {Q_META, "api_version", Q_APIVER}, {Q_META, "billed_units", Q_BILLED}, {Q_META, "tokens", Q_TOKENS}, {Q_META, "cached_tokens", Q_F64}, {Q_META, "warnings", Q_STRS},
+  {Q_APIVER, "version", Q_STR}, {Q_APIVER, "is_deprecated", Q_BOOL}, {Q_APIVER, "is_experimental", Q_BOOL},
+  {Q_BILLED, "images", Q_F64}, {Q_BILLED, "input_tokens", Q_F64}, {Q_BILLED, "output_tokens", Q_F64}, {Q_BILLED, "search_units", Q_F64}, {Q_BILLED, "classifications", Q_F64},
+  {Q_TOKENS, "input_tokens", Q_IN}, {Q_TOKENS, "output_tokens", Q_OUT},
+};
+static constexpr int kNumRerankFields = sizeof(kRerankFields) / sizeof(kRerankFields[0]);
+static_assert(kNumRerankFields <= 64 && Q_COUNT <= N_COUNT, "the rerank schema uses a SchemaBlob");
+
+static inline SchemaBlob build_rerank_schema() {
+  SchemaBlob b; memset(&b, 0, sizeof b);
+  auto set = [&](int n, uint8_t kind, uint8_t cap = NOCAP, uint8_t elem = 0) { b.nodes[n].kind = kind; b.nodes[n].cap = cap; b.nodes[n].elem = elem; };
+  set(Q_ANY, K_ANY); set(Q_STR, K_STR); set(Q_INT, K_INT); set(Q_F64, K_F64); set(Q_BOOL, K_BOOL);
+  set(Q_ROOT, K_OBJ); set(Q_RESULTS, K_ARR, NOCAP, Q_RESULT); set(Q_RESULT, K_OBJ); set(Q_META, K_OBJ); set(Q_APIVER, K_OBJ); set(Q_BILLED, K_OBJ);
+  set(Q_TOKENS, K_OBJ, C_OBJ_USAGE); set(Q_STRS, K_ARR, NOCAP, Q_STR);
+  set(Q_IN, K_F64, C_PROMPT); set(Q_OUT, K_F64, C_COMPLETION);
+  int ko = 0;
+  for (int f = 0; f < kNumRerankFields; f++) {
+    const FieldDef& d = kRerankFields[f];
+    Node& o = b.nodes[d.owner];
+    if (o.nf == 0) o.f0 = (uint8_t)f;   // fields of one owner are contiguous in kRerankFields
+    o.nf++;
+    int kl = (int)strlen(d.key);
+    b.fields[f].koff = (uint16_t)ko; b.fields[f].klen = (uint8_t)kl; b.fields[f].node = d.node;
+    memcpy(b.keys + ko, d.key, kl); ko += kl;
+  }
+  return b;
+}
+
 // ------------------------------------------------------------------ R1: non-stream ChatCompletionResponse usage
 // json.NewDecoder(body).Decode(&openai.ChatCompletionResponse{}) then usage / model
 // (internal/translator/openai_openai.go:146-174; struct internal/apischema/openai/openai.go:1269-1306,1365-1422).

@@ -13,13 +13,16 @@ namespace aigw { namespace tj {
 
 enum Kind : uint8_t { K_ANY = 0, K_STR, K_INT, K_FLOAT, K_BOOL, K_OBJ, K_ARR, K_CREATED, K_B64, K_STROBJ /* string, or the object node in `elem` */,
                       K_MAP /* map[string]T: an object with arbitrary keys whose values are all of node `elem` */,
-                      // the kinds below are walked only by walk<CAP, true> (the Responses API schema); the other schemas compile without them
+                      // the kinds below are walked only by walk<CAP, true> (the Responses API schema) and K_F64 only by walk<CAP, EXT, true>
+                      // (the rerank schema); the other schemas compile without them
                       K_UNION /* tagged union: an object whose first top-level "type" string picks the variant node from the tag table
                                  fields[f0, f0+nf) (key = tag); null, a non-object, an unknown tag or a missing / non-string "type" fail */,
                       K_STRARR /* a string, or the array node in `elem`; anything else, null included, fails */,
                       K_DECLINE /* a member the schema knows but does not restate: any value sets `weird` */,
                       K_PCREATED /* *JSONUNIXTime: null is nil, anything else as K_CREATED */,
-                      K_F32 /* float32: a number; an exponent or more than 38 integer digits (range not restated) sets `weird` */ };
+                      K_F32 /* float32: a number; an exponent or more than 38 integer digits (range not restated) sets `weird` */,
+                      K_F64 /* float64: a number; an exponent or more than 308 integer digits (overflow not restated) sets `weird`.  With a
+                               capture, ints[cap] = uint32(float64(text)) (f64_trunc_u32; `weird` when that is not defined) */ };
 
 struct Field { uint16_t koff; uint8_t klen; uint8_t node; };  // key bytes at keys[koff..koff+klen)
 struct Node { uint8_t kind; uint8_t cap; uint8_t f0; uint8_t nf; uint8_t elem; };
@@ -86,6 +89,41 @@ __device__ inline bool parse_i64(const uint8_t* p, int b, int e, uint32_t& low32
   if (neg) { if (v > 0x8000000000000000ull) return false; low32 = (uint32_t)(0ull - v); }
   else { if (v > 0x7FFFFFFFFFFFFFFFull) return false; low32 = (uint32_t)v; }
   if (big) *big = neg ? v != 0 : (v >> 31) != 0;
+  return true;
+}
+
+// uint32(float64(text)) for a number without exponent whose integer digits are p[b, ie) (b after an optional '-') and whose
+// fraction digits, if any, are p[ie + 1, j).  Go truncates toward zero after rounding the text to the nearest float64, so the result
+// is the integer part I, or I + 1 when the text rounds up to it.  That happens iff the fraction is >= 1 - 2^-q: the float64s just
+// below I + 1 are 2^(floor(log2 I) - 52) apart (2^-53 below 1), q = 53 - floor(log2 I) (54 for I = 0), and the tie goes to I + 1,
+// whose mantissa is even.  1 - 2^-q has q decimals, so the test reads the first q fraction digits F (zero-padded): F >= 10^q - 5^q,
+// i.e. the nines' complement of F is below 5^q < 10^38.  false: the rounded value lies outside (-1, 2^32), where Go's conversion is
+// implementation-defined.
+__device__ inline bool f64_trunc_u32(const uint8_t* p, int i, int ie, int j, uint32_t& out) {
+  const bool neg = p[i] == '-';
+  const int b = i + (neg ? 1 : 0);
+  if (ie - b > 10) return false;
+  unsigned long long I = 0;
+  for (int k = b; k < ie; k++) I = I * 10ull + (p[k] - '0');
+  if (I > 0xffffffffull || (neg && I)) return false;
+  if (ie < j) {
+    int fl = 0;   // floor(log2 I); a loop rather than __clzll so that the host build of the walker compiles too
+    for (unsigned long long t = I; t > 1; t >>= 1) fl++;
+    const int f0 = ie + 1, q = I ? 53 - fl : 54;
+    bool up = true;
+    unsigned __int128 c = 0, five = 1;
+    for (int k = 0; k < q; k++) {
+      const uint32_t cd = 9u - (f0 + k < j ? (uint32_t)(p[f0 + k] - '0') : 0u);
+      if (k < q - 38) { if (cd) { up = false; break; } }
+      else c = c * 10u + cd;
+      five *= 5u;
+    }
+    if (up && c < five) {
+      if (neg || I == 0xffffffffull) return false;   // -1.0, 2^32
+      I++;
+    }
+  }
+  out = (uint32_t)I;
   return true;
 }
 
@@ -172,8 +210,9 @@ __device__ inline int union_tag(const uint8_t* p, int i, int n, int& ts, int& tl
 }
 
 // Typed walk of p[0..n).  Returns true when json.Unmarshal into the schema's root type would succeed.  EXT: the schema uses the
-// kinds from K_UNION on.
-template <class CAP, bool EXT = false>
+// kinds from K_UNION to K_F32.  F64: the schema uses K_F64 (a separate flag: its exact conversion would otherwise enlarge the
+// stack frame of every EXT walk).
+template <class CAP, bool EXT = false, bool F64 = false>
 __device__ inline bool walk(const uint8_t* p, int n, const Node* nodes, const Field* fields, const char* keys, int root, CAP& cap, bool allow_trailing = false) {
   const int MAXD = 12;
   uint8_t st_node[MAXD]; uint32_t st_seen[MAXD];
@@ -208,6 +247,18 @@ __device__ inline bool walk(const uint8_t* p, int n, const Node* nodes, const Fi
         nd.kind = K_FLOAT;
         bool ii; int ie; const int j = (c == '-' || dig(c)) ? scan_number(p, i, n, ii, ie) : -1;
         if (j >= 0) { bool ex = false; for (int k = ie; k < j; k++) ex |= (p[k] | 0x20) == 'e'; if (ex || ie - i - (c == '-') > 38) cap.weird = 1; }
+      }
+    }
+    if constexpr (F64) {
+      if (nd.kind == K_F64) {
+        const uint8_t fc = nd.cap; nd.kind = K_FLOAT; nd.cap = 0xff;
+        bool ii; int ie; const int j = (c == '-' || dig(c)) ? scan_number(p, i, n, ii, ie) : -1;
+        if (j >= 0) {
+          bool ex = false; for (int k = ie; k < j; k++) ex |= (p[k] | 0x20) == 'e';
+          uint32_t v;
+          if (ex || ie - i - (c == '-') > 308) cap.weird = 1;
+          else if (fc != 0xff) { if (!f64_trunc_u32(p, i, ie, j, v)) cap.weird = 1; else { cap.ints[fc] = v; cap.int_set |= 1u << fc; } }
+        }
       }
     }
     bool descend = false;

@@ -115,7 +115,29 @@ enum aigw_schema { AIGW_SCHEMA_OPENAI = 0, AIGW_SCHEMA_AWS_BEDROCK = 1, AIGW_SCH
                     * DECLINED: a null root, "prompt":null, escaped keys and model, repeated known keys, float64 values (members, numbers
                     * in stop) with an exponent or more than 308 integer digits.  A token-id prompt costs two index tokens per id, so long ones decline with
                     * AIGW_R_TOKENS (DESIGN.md §7). */
-                   AIGW_SCHEMA_COMPLETIONS = 256, AIGW_SCHEMA_COMPLETIONS_OPENAI = 256 };
+                   AIGW_SCHEMA_COMPLETIONS = 256, AIGW_SCHEMA_COMPLETIONS_OPENAI = 256,
+                   /* Cohere (filterapi.APISchemaCohere): a base schema of its own.  Alone it is no chat schema (DECLINED, AIGW_R_SCHEMA). */
+                   AIGW_SCHEMA_COHERE = 7,
+                   /* Cohere /v2/rerank requests: RerankEndpointSpec.ParseBody (endpointspec.go:364-373, json.Unmarshal into
+                    * cohere.RerankV2Request) + cohereToCohereTranslatorV2Rerank.RequestBody (cohere_rerank_v2.go:40-66).
+                    * AIGW_SCHEMA_RERANK | base schema; only the Cohere base has a translator (GetTranslator, endpointspec.go:376-383),
+                    * every other base is DECLINED (AIGW_R_SCHEMA).  Result: model span = ParseBody's model, flags 0 (rerank never
+                    * streams), record = [":path" = path.Join("/", api_version, "rerank"), "/rerank" when api_version is empty or NULL;
+                    * the version is cleaned as path.Join cleans it: "." / ".." segments and doubled slashes; a path above 128 bytes is
+                    * DECLINED][body]; body_kind UNCHANGED,
+                    * or BYTES with model_name_override (sjson set of "model": the first value spliced, or the member appended at the
+                    * root) or force_body_mutation (the original bytes, onRetry).  Every member is type-checked as the decoder does (a type
+                    * error is AIGW_MALFORMED_400, unknown keys such as return_documents / rank_fields are skipped, ranges are not
+                    * checked): model / query strings, documents an array of strings (null elements allowed), top_n /
+                    * max_tokens_per_doc int64 (exact range; a fraction or exponent is a 400); null is accepted for each.  DECLINED: a
+                    * null root, escaped keys and model, repeated known keys.  Each document costs index tokens, so requests with very
+                    * many short documents decline with AIGW_R_TOKENS (DESIGN.md §7); bodies above 64 KiB with AIGW_R_TOO_LARGE. */
+                   AIGW_SCHEMA_RERANK = 512, AIGW_SCHEMA_RERANK_COHERE = 519,
+                   /* cohereToCohereTranslatorV2Rerank.ResponseError (cohere_rerank_v2.go:110-135): with force_body_mutation (the
+                    * upstream content-type is present and not JSON) the raw body becomes {"message":"<body as a JSON string>"}
+                    * (json.Marshal of RerankV2Error); otherwise the body is forwarded untouched (DECLINED, do not call).  Bodies with a
+                    * byte >= 0x80 and empty bodies are DECLINED (the reference answers {"message":""} for an empty one). */
+                   AIGW_SCHEMA_RESP_ERROR_COHERE = 31 };
 
 /* Why a body was declined / rejected (diagnostics; stable numbering). */
 enum aigw_reason {
@@ -283,6 +305,19 @@ int aigw_responses_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies,
                                          aigw_sse_result* d_results, void* stream, float* kernel_ms);
 int aigw_responses_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
                                        aigw_sse_result* results, const int32_t* cost_types, uint32_t n_costs, uint64_t* costs /* n * n_costs, may be NULL */);
+/* Same for Cohere /v2/rerank: cohereToCohereTranslatorV2Rerank.ResponseBody (internal/translator/cohere_rerank_v2.go:73-108) —
+ * json.NewDecoder(body).Decode(&cohere.RerankV2Response{}): the first JSON value counts and trailing bytes are ignored; an empty or
+ * white-space-only body, or a member of the wrong type, is AIGW_INTERNAL ("failed to unmarshal body").  Every member is type-checked:
+ * results ([]*{index int, relevance_score float64}, null elements allowed), id, meta.api_version {version, is_deprecated,
+ * is_experimental}, meta.billed_units (five float64), meta.tokens, meta.cached_tokens, meta.warnings ([]string).  A non-null
+ * meta.tokens sets total (mask bit 2), input_tokens sets input (bit 0) and output_tokens sets output (bit 1) when non-null; each count
+ * is uint32(float64(text)) (truncation toward zero, computed exactly from the text) and total is their uint32 sum.  model_len is
+ * always 0: the reference reports the request model.  AIGW_DECLINED: a float64 with an exponent or more than 308 integer digits,
+ * a token count outside (-1, 2^32) after rounding, escaped or repeated keys. */
+int aigw_rerank_response_usage_device(aigw_ctx* ctx, const uint8_t* d_bodies, const uint64_t* d_offsets, const uint32_t* d_lens, uint32_t n,
+                                      aigw_sse_result* d_results, void* stream, float* kernel_ms);
+int aigw_rerank_response_usage_host(aigw_ctx* ctx, const uint8_t* bodies, const uint64_t* offsets, const uint32_t* lens, uint32_t n,
+                                    aigw_sse_result* results, const int32_t* cost_types, uint32_t n_costs, uint64_t* costs /* n * n_costs, may be NULL */);
 int aigw_usage_costs_device(aigw_ctx* ctx, const aigw_sse_result* d_results, uint32_t n, const int32_t* d_cost_types, uint32_t n_costs,
                             uint64_t* d_costs, void* stream);
 
