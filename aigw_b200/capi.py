@@ -44,7 +44,7 @@ assert MutResult.itemsize == 16
 EXPORTS = ["aigw_bind_numa", "aigw_stream_open", "aigw_stream_open_batch", "aigw_stream_chunks", "aigw_stream_chunks_soa", "aigw_stream_chunk", "aigw_stream_close", "aigw_stream_close_batch",
            "aigw_version", "aigw_init", "aigw_destroy", "aigw_last_error", "aigw_device_sm_count", "aigw_host_alloc", "aigw_host_free",
            "aigw_device_alloc", "aigw_device_free", "aigw_memcpy_h2d", "aigw_memcpy_d2h", "aigw_memset_d", "aigw_sync",
-           "aigw_chat_translate_device", "aigw_chat_translate_device_mapped", "aigw_chat_last_profile", "aigw_chat_set_profile", "aigw_chat_set_small_batch", "aigw_chat_translate_host", "aigw_sse_usage_device", "aigw_sse_usage_host", "aigw_response_usage_device", "aigw_response_usage_host", "aigw_embeddings_response_usage_device", "aigw_embeddings_response_usage_host", "aigw_completions_response_usage_device", "aigw_completions_response_usage_host", "aigw_responses_response_usage_device", "aigw_responses_response_usage_host", "aigw_rerank_response_usage_device", "aigw_rerank_response_usage_host", "aigw_usage_costs_device",
+           "aigw_chat_translate_device", "aigw_chat_translate_device_mapped", "aigw_chat_last_profile", "aigw_chat_set_profile", "aigw_chat_set_small_batch", "aigw_chat_translate_host", "aigw_rerank_translate_large_device", "aigw_rerank_translate_large_host", "aigw_sse_usage_device", "aigw_sse_usage_host", "aigw_response_usage_device", "aigw_response_usage_host", "aigw_embeddings_response_usage_device", "aigw_embeddings_response_usage_host", "aigw_completions_response_usage_device", "aigw_completions_response_usage_host", "aigw_responses_response_usage_device", "aigw_responses_response_usage_host", "aigw_rerank_response_usage_device", "aigw_rerank_response_usage_host", "aigw_usage_costs_device",
            "aigw_bedrock_stream_device", "aigw_bedrock_stream_host", "aigw_body_mutate_device", "aigw_body_mutate_host",
            "aigw_cost_compile", "aigw_cost_program_free", "aigw_usage_costs_cel_device", "aigw_usage_costs_cel_host", "aigw_sha256_device", "aigw_chat_body_sha256_device", "aigw_sha256_host", "aigw_bpe_load", "aigw_bpe_free", "aigw_bpe_count_device", "aigw_bpe_count_host", "aigw_embeddings_count_device", "aigw_embeddings_count_host", "aigw_batcher_start", "aigw_batcher_add_backend", "aigw_batcher_translate", "aigw_batcher_translate_to", "aigw_batcher_get_stats", "aigw_batcher_stop"]
 
@@ -120,6 +120,8 @@ def load_library():
     L.aigw_chat_set_profile.argtypes = [C.c_void_p, C.c_int]
     L.aigw_chat_set_small_batch.argtypes = [C.c_void_p, C.c_int]; L.aigw_chat_set_small_batch.restype = None
     L.aigw_chat_translate_host.argtypes = [C.c_void_p, C.POINTER(BackendCfg), C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(_BatchOut)]
+    L.aigw_rerank_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
+    L.aigw_rerank_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
     L.aigw_sse_usage_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
     L.aigw_sse_usage_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64),
                                       C.POINTER(C.c_uint64), C.POINTER(C.c_float)]
@@ -241,9 +243,13 @@ class Context:
 
     # ---- chat translate, host buffers (the call the shim makes)
     def chat_translate_host(self, cfg, arena, offs, lens):
+        return self._translate_host(self.L.aigw_chat_translate_host, "chat_translate_host", cfg, arena, offs, lens)
+
+    def _translate_host(self, fn, what, cfg, arena, offs, lens):
+        """a host-buffer call with the aigw_chat_translate_host signature → (results view, output arena view, stats)"""
         out = _BatchOut()
         n = len(lens)
-        self._check(self.L.aigw_chat_translate_host(self.h, C.byref(cfg), arena.ctypes.data, offs.ctypes.data, lens.ctypes.data, n, C.byref(out)), "chat_translate_host")
+        self._check(fn(self.h, C.byref(cfg), arena.ctypes.data, offs.ctypes.data, lens.ctypes.data, n, C.byref(out)), what)
         res = np.ctypeslib.as_array((C.c_uint8 * (n * 32)).from_address(out.results)).view(DocResult) if n else np.zeros(0, DocResult)
         arena_out = np.ctypeslib.as_array((C.c_uint8 * max(1, out.out_used)).from_address(out.out)) if out.out_used else np.zeros(0, np.uint8)
         stats = {"h2d_bytes": out.h2d_bytes, "d2h_bytes": out.d2h_bytes, "gpu_launches": out.gpu_launches, "kernel_ms": out.kernel_ms}
@@ -253,6 +259,27 @@ class Context:
         """Convenience for tests: list of bytes → list of (status, reason, path, body, model, stream)."""
         arena, offs, lens = pack_bodies(bodies)
         res, out, _ = self.chat_translate_host(cfg, arena, offs, lens)
+        return self._records(bodies, res, out)
+
+    # ---- Cohere /v2/rerank requests of any size below 16 MiB (one CTA streams one request)
+    def rerank_translate_large_host(self, cfg, arena, offs, lens):
+        """Same results as chat_translate_host under the rerank schema, for bodies of 1 byte to 16 MiB - 1."""
+        return self._translate_host(self.L.aigw_rerank_translate_large_host, "rerank_translate_large_host", cfg, arena, offs, lens)
+
+    def rerank_translate_large(self, cfg, bodies):
+        """list of bytes → the same dicts as chat_translate"""
+        arena, offs, lens = pack_bodies(bodies)
+        res, out, _ = self.rerank_translate_large_host(cfg, arena, offs, lens)
+        return self._records(bodies, res, out)
+
+    def rerank_translate_large_device(self, cfg, d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used, timed=True):
+        ms = C.c_float(0)
+        self._check(self.L.aigw_rerank_translate_large_device(self.h, C.byref(cfg), d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used, None,
+                                                              C.byref(ms) if timed else None), "rerank_translate_large_device")
+        return ms.value
+
+    @staticmethod
+    def _records(bodies, res, out):
         r = []
         for i in range(len(bodies)):
             x = res[i]

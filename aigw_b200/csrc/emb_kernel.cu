@@ -20,6 +20,7 @@
 #include "emb_kernel.cuh"
 
 #include "classify.cuh"
+#include "scan_common.cuh"
 
 namespace aigw {
 
@@ -28,8 +29,6 @@ static constexpr uint32_t kTile = kEmbThreads * 32;
 enum : uint32_t { T_QOPEN = '"', T_QCLOSE = '\'', T_SCALAR = 's' };
 static constexpr uint32_t kNoFail = 0xffffffffu;
 
-__device__ __forceinline__ uint32_t prefix_xor32(uint32_t x) { x ^= x << 1; x ^= x << 2; x ^= x << 4; x ^= x << 8; x ^= x << 16; return x; }
-
 struct EmbShared {
   uint32_t wpar[2][8], wlast[2][8], wcnt[2][8];
   uint32_t doc; uint32_t fail;   // lowest reason code raised by any thread (declines, below 32, win over the definite errors); kNoFail = none
@@ -37,31 +36,6 @@ struct EmbShared {
   uint32_t text_base, n_inputs, str_open, str_close;
   uint32_t n_blank;   // rows below the text table's capacity that a request straddling it was handed (written as empty texts)
 };
-
-// JSON scalar in [p, p+n): 0 invalid, 1 null, 2 true / false, 3 integer (-?digits, at most 18), 4 other number
-__device__ int emb_scalar_kind(const uint8_t* p, uint32_t n) {
-  if (n == 4 && p[0] == 'n' && p[1] == 'u' && p[2] == 'l' && p[3] == 'l') return 1;
-  if (n == 4 && p[0] == 't' && p[1] == 'r' && p[2] == 'u' && p[3] == 'e') return 2;
-  if (n == 5 && p[0] == 'f' && p[1] == 'a' && p[2] == 'l' && p[3] == 's' && p[4] == 'e') return 2;
-  uint32_t i = 0;
-  if (i < n && p[i] == '-') i++;
-  const uint32_t d0 = i;
-  if (i >= n) return 0;
-  if (p[i] == '0') i++;
-  else if (p[i] >= '1' && p[i] <= '9') { while (i < n && p[i] >= '0' && p[i] <= '9') i++; }
-  else return 0;
-  const uint32_t nd = i - d0;
-  if (i == n) return nd <= 18 ? 3 : 4;
-  if (p[i] == '.') { i++; const uint32_t f0 = i; while (i < n && p[i] >= '0' && p[i] <= '9') i++; if (i == f0) return 0; }
-  if (i < n && (p[i] == 'e' || p[i] == 'E')) { i++; if (i < n && (p[i] == '+' || p[i] == '-')) i++; const uint32_t e0 = i; while (i < n && p[i] >= '0' && p[i] <= '9') i++; if (i == e0) return 0; }
-  return i == n ? 4 : 0;
-}
-
-__device__ __forceinline__ bool emb_key_is(const uint8_t* p, uint32_t n, const char* k, uint32_t kl) {
-  if (n != kl) return false;
-  for (uint32_t i = 0; i < n; i++) if (p[i] != (uint8_t)k[i]) return false;
-  return true;
-}
 
 __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanParams P) {
   __shared__ EmbShared S;
@@ -192,7 +166,7 @@ __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanP
       else for (;;) {
         if (ty(j) != T_QOPEN || ty(j + 1) != T_QCLOSE || ty(j + 2) != ':') { f = AIGW_R_E400_SYNTAX; break; }
         const uint8_t* kp = body + ps(j) + 1u; const uint32_t kl = ps(j + 1) - ps(j) - 1u;
-        int id = emb_key_is(kp, kl, "model", 5) ? 0 : emb_key_is(kp, kl, "input", 5) ? 1 : emb_key_is(kp, kl, "encoding_format", 15) ? 2 : emb_key_is(kp, kl, "dimensions", 10) ? 3 : emb_key_is(kp, kl, "user", 4) ? 4 : -1;
+        int id = scan_key_is(kp, kl, "model", 5) ? 0 : scan_key_is(kp, kl, "input", 5) ? 1 : scan_key_is(kp, kl, "encoding_format", 15) ? 2 : scan_key_is(kp, kl, "dimensions", 10) ? 3 : scan_key_is(kp, kl, "user", 4) ? 4 : -1;
         if (id < 0) { f = AIGW_R_UNSUPPORTED_FIELD; break; }
         if (seen & (1u << id)) { f = AIGW_R_DUP_KEY; break; }
         seen |= 1u << id;
@@ -204,7 +178,7 @@ __global__ void __launch_bounds__(kEmbThreads, 4) emb_scan_kernel(const EmbScanP
           if (v + 1 >= ntok) { f = AIGW_R_E400_SYNTAX; break; }
           uint32_t e = ps(v + 1); const uint32_t b = ps(v);
           while (e > b && (body[e - 1] == ' ' || body[e - 1] == '\n' || body[e - 1] == '\r' || body[e - 1] == '\t')) e--;
-          const int sk = emb_scalar_kind(body + b, e - b);
+          const int sk = scan_scalar_kind(body + b, e - b);
           if (!sk) { f = AIGW_R_E400_SYNTAX; break; }
           kind = sk; next = v + 1;
         }

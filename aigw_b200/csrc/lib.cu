@@ -23,6 +23,7 @@
 #include "stream_kernel.cuh"
 #include "bpe_kernel.cuh"
 #include "emb_kernel.cuh"
+#include "rerank_large_kernel.cuh"
 
 #include <mutex>
 
@@ -100,6 +101,8 @@ struct aigw_ctx {
   long small_max = -1;   // aigw_chat_set_small_batch; -1: AIGW_SMALL_MAX or 512
   // large embeddings requests (aigw_embeddings_count_device): token workspace, text table, counts
   Scratch<uint32_t> d_emb_tok; Scratch<uint64_t> d_emb_toff; Scratch<uint32_t> d_emb_tlen; Scratch<uint32_t> d_emb_cnt;
+  // large rerank requests (aigw_rerank_translate_large_device): token and depth workspace, splice table
+  Scratch<uint32_t> d_rr_tok; Scratch<uint8_t> d_rr_dep; Scratch<RerankSplice> d_rr_splice;
   PinnedScratch<uint8_t> h_small;   // small-batch path: tables + bodies, read by the kernel in place
   // chat workspace (intermediates of one sub-batch) + per-stage timing events
   Scratch<uint8_t> d_work;
@@ -809,6 +812,76 @@ int aigw_embeddings_count_host(aigw_ctx* ctx, const aigw_bpe* bpe, const uint8_t
 }
 
 // ------------------------------------------------------------------ SSE
+// ------------------------------------------------------------------ Cohere /v2/rerank requests of any size below 16 MiB
+int aigw_rerank_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                       const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                       aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  if (!ctx) return -2;
+  if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
+  ENTER_ON(stream);
+  ChatParams C;
+  fill_params(C, cfg);   // the cleaned ":path" and the override, exactly as the translate pass gets them
+  RerankLargeParams P;
+  P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.results = d_results;
+  P.out = d_out; P.out_capacity = out_capacity; P.out_used = (unsigned long long*)d_out_used;
+  P.call_reason = (!cfg || cfg->schema != AIGW_SCHEMA_RERANK_COHERE) ? AIGW_R_SCHEMA : C.prefix_len == 0 ? AIGW_R_UNSUPPORTED_FIELD : 0;
+  P.force_mutation = C.force_mutation ? 1u : 0u;
+  P.override_len = C.override_len;
+  P.override_ok = 1;
+  for (uint32_t i = 0; i < C.override_len; i++) { const uint32_t c = (uint8_t)C.override_model[i]; if (c < 0x20 || c > 0x7f || c == '"' || c == '\\') P.override_ok = 0; }
+  P.path_len = C.prefix_len;
+  memcpy(P.override_model, C.override_model, sizeof P.override_model);
+  memcpy(P.path, C.openai_path, sizeof P.path);
+  P.tok_cap = rerank_tok_cap(max_len && max_len < (1u << 24) ? max_len : (1u << 24) - 1u);
+  const int grid = rerank_scan_grid(ctx->sm_count, P.tok_cap);
+  CK(ctx->d_rr_tok.ensure((size_t)grid * P.tok_cap * 4));
+  CK(ctx->d_rr_dep.ensure((size_t)grid * P.tok_cap));
+  CK(ctx->d_rr_splice.ensure((size_t)n * sizeof(RerankSplice)));
+  P.tok_ws = ctx->d_rr_tok; P.dep_ws = ctx->d_rr_dep; P.splice = ctx->d_rr_splice;
+  unsigned int* c0;
+  if (int rc = take_counters(ctx, 2, st, &c0)) return rc;
+  P.next_scan = c0; P.next_emit = c0 + 1;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_rerank_large(P, ctx->sm_count, st)); return 0; });
+}
+
+int aigw_rerank_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                     const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  memset(out, 0, sizeof *out);
+  if (!ctx) return -2;
+  if (n == 0) return 0;
+  ENTER();
+  ChatParams C;
+  fill_params(C, cfg);
+  // every record fits its slot: the path, the body, and the override with the ,"model":"" around it
+  uint32_t max_len = 0;
+  uint64_t cap = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (offsets[i] & 15u) { ctx->err = "aigw_rerank_translate_large_host: request starts must be 16-byte aligned"; return -2; }
+    if (lens[i] > max_len) max_len = lens[i];
+    cap += ((uint64_t)C.prefix_len + lens[i] + C.override_len + 16u + 15u) & ~15ull;
+  }
+  HostStage S(ctx);
+  const uint8_t* d_bodies = S.span(bodies, offsets, lens, n);
+  const uint64_t* d_off = S.in(offsets, n);
+  const uint32_t* d_len = S.in(lens, n);
+  uint8_t* d_out = S.out<uint8_t>(cap);
+  aigw_doc_result* d_res = S.out<aigw_doc_result>(n);
+  uint64_t* d_used = S.out<uint64_t>(1);
+  S.step([&] { CK(cudaMemsetAsync(d_used, 0, 8, S.st)); return 0; });
+  S.step([&] { CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result))); CK(ctx->h_out.ensure(cap)); CK(ctx->h_used_arr.ensure(8)); return 0; });
+  if (S.rc) return S.rc;
+  float ms = 0;
+  if (int rc = aigw_rerank_translate_large_device(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
+  S.back(ctx->h_res.p, d_res, n);
+  S.back((uint64_t*)ctx->h_used_arr.p, d_used, 1);
+  if (int rc = S.wait()) return rc;
+  const uint64_t used = ctx->h_used_arr[0] < cap ? ctx->h_used_arr[0] : cap;
+  if (used) { CK(cudaMemcpyAsync(ctx->h_out, d_out, used, cudaMemcpyDeviceToHost, S.st)); CK(cudaStreamSynchronize(S.st)); }
+  out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = S.h2d + 8; out->d2h_bytes = S.d2h + used;
+  out->gpu_launches = 2; out->kernel_ms = ms;
+  return 0;
+}
+
 int aigw_sse_usage_device(aigw_ctx* ctx, const uint8_t* d_bytes, const uint64_t* d_chunk_off, const uint32_t* d_chunk_first,
                           uint32_t n_streams, aigw_sse_result* d_results, void* stream, float* kernel_ms) {
   if (n_streams == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }

@@ -131,7 +131,8 @@ enum aigw_schema { AIGW_SCHEMA_OPENAI = 0, AIGW_SCHEMA_AWS_BEDROCK = 1, AIGW_SCH
                     * checked): model / query strings, documents an array of strings (null elements allowed), top_n /
                     * max_tokens_per_doc int64 (exact range; a fraction or exponent is a 400); null is accepted for each.  DECLINED: a
                     * null root, escaped keys and model, repeated known keys.  Each document costs index tokens, so requests with very
-                    * many short documents decline with AIGW_R_TOKENS (DESIGN.md §7); bodies above 64 KiB with AIGW_R_TOO_LARGE. */
+                    * many short documents decline with AIGW_R_TOKENS (DESIGN.md §7); bodies above 64 KiB with AIGW_R_TOO_LARGE
+                    * (aigw_rerank_translate_large_* takes those). */
                    AIGW_SCHEMA_RERANK = 512, AIGW_SCHEMA_RERANK_COHERE = 519,
                    /* cohereToCohereTranslatorV2Rerank.ResponseError (cohere_rerank_v2.go:110-135): with force_body_mutation (the
                     * upstream content-type is present and not JSON) the raw body becomes {"message":"<body as a JSON string>"}
@@ -258,6 +259,29 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
  * window.  Default 512 (AIGW_SMALL_MAX overrides); 0 sends every call through the throughput pipeline; -1 restores the default.
  * Both paths produce the same bytes (same stage code). */
 void aigw_chat_set_small_batch(aigw_ctx* ctx, int max_docs);
+
+/* ---- Cohere /v2/rerank requests of any size below 16 MiB ----
+ * The translate pass holds a body in one warp's shared memory, so aigw_chat_translate_* declines every AIGW_SCHEMA_RERANK_COHERE
+ * body above 64 KiB (AIGW_R_TOO_LARGE); a RAG rerank of many retrieved chunks is larger.  These calls stream one request through
+ * one CTA and give exactly the AIGW_SCHEMA_RERANK_COHERE results of aigw_chat_translate_* (same ":path", model span, flags 0,
+ * body_kind, 400s, declines, override check; members checked in body order), for bodies of 1 byte to 16 MiB - 1 (small ones
+ * included).  Arguments, records and results are those of aigw_chat_translate_device / _host; `cfg->schema` other than
+ * AIGW_SCHEMA_RERANK_COHERE declines every body with AIGW_R_SCHEMA.  Further declines:
+ *   AIGW_R_TOO_LARGE   a body of 16 MiB or more, or a model string above 65535 bytes (model_len is 16 bits)
+ *   AIGW_R_TOKENS      a body with more than len / 4 + 1024 scan tokens (structural bytes outside strings, both quotes of every
+ *                      string, the first byte of every scalar): each slice of the token workspace holds that many for the call's
+ *                      longest body (max_len; 0 = unknown: sized for 16 MiB)
+ *   AIGW_R_DEPTH       nesting deeper than 48
+ *   AIGW_R_OUT_SPACE   (device form) the record does not fit out_capacity; records are bump-allocated in the order requests
+ *                      finish, so which ones do not fit depends on that order.  align16(path_len + len + override_len + 16) per
+ *                      body is always enough.
+ * The host form is a staging wrapper around the device form: it sizes the output arena that way itself; `out` stays valid until
+ * the next host-buffer call on the context.  Offsets must be multiples of 16. */
+int aigw_rerank_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                       const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                       aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+int aigw_rerank_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                     const uint32_t* lens, uint32_t n, aigw_batch_out* out);
 
 /* ---- OpenAI SSE response streams: usage scan (S1) + TokenUsage merge (C1) ----
  * Stream s consists of chunks [chunk_first[s], chunk_first[s+1]); chunk c is bytes

@@ -15,6 +15,7 @@ import "C"
 
 import (
 	"errors"
+	"sync"
 	"unsafe"
 )
 
@@ -25,6 +26,10 @@ var ErrDeclined = errors.New("gpupipeline: declined")
 type Pipeline struct {
 	ctx     *C.aigw_ctx
 	batcher *C.aigw_batcher
+	// bulk: a second context for the host-buffer calls the shim makes itself (TranslateRerank), so that they never meet the
+	// batcher's own host-buffer calls on ctx; one call at a time under bulkMu
+	bulk   *C.aigw_ctx
+	bulkMu sync.Mutex
 }
 
 // Backend indexes a backend registered with the batcher (one per filterapi.Backend schema / override combination).
@@ -39,6 +44,11 @@ func New(device int, maxBatch, windowMicros uint32, first C.aigw_backend_cfg) (*
 	if rc := C.aigw_batcher_start(p.ctx, &first, C.uint32_t(maxBatch), C.uint32_t(windowMicros), &p.batcher); rc != 0 {
 		C.aigw_destroy(p.ctx)
 		return nil, errors.New("aigw_batcher_start failed")
+	}
+	if rc := C.aigw_init(C.int(device), &p.bulk); rc != 0 {
+		C.aigw_batcher_stop(p.batcher)
+		C.aigw_destroy(p.ctx)
+		return nil, errors.New("aigw_init failed")
 	}
 	return p, nil
 }
@@ -84,6 +94,47 @@ func (p *Pipeline) Translate(be Backend, body, scratch []byte) (Result, error) {
 		return r, nil // 400 / 422 / internal: internalapi.ErrMalformedRequest / ErrInvalidRequestBody, as today
 	}
 	pl, bl := int(res.path_len), int(res.body_len)
+	r.Path = scratch[:pl]
+	if !r.Unchanged {
+		r.Body = scratch[pl : pl+bl]
+	}
+	r.Model = body[int(res.model_off) : int(res.model_off)+int(res.model_len)]
+	return r, nil
+}
+
+// RerankBatcherMax is the largest Cohere /v2/rerank body the batcher's translate pass holds; larger ones go to
+// aigw_rerank_translate_large_host (TranslateRerank).
+const RerankBatcherMax = 65536
+
+// TranslateRerank is Translate for a backend registered with RerankRequestSchema: a body of up to RerankBatcherMax bytes joins
+// the backend's batch as before, a larger one (a RAG rerank of many retrieved chunks, up to 16 MiB - 1) is streamed through one
+// CTA by aigw_rerank_translate_large_host with the same semantics.  cfg is the configuration the backend was registered with.
+// The large call's record lives in the context's pinned arena, so it is copied into scratch, which must hold
+// len(body) + len(model override) + 160 bytes; a smaller scratch declines.
+func (p *Pipeline) TranslateRerank(be Backend, cfg *C.aigw_backend_cfg, body, scratch []byte) (Result, error) {
+	if len(body) <= RerankBatcherMax {
+		return p.Translate(be, body, scratch)
+	}
+	off, ln := C.uint64_t(0), C.uint32_t(len(body))
+	var out C.aigw_batch_out
+	p.bulkMu.Lock()
+	defer p.bulkMu.Unlock()
+	if rc := C.aigw_rerank_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	res := *out.results
+	r := Result{Status: int(res.status), Reason: int(res.reason), Unchanged: res.body_kind == C.AIGW_BODY_UNCHANGED}
+	if res.status == C.AIGW_DECLINED {
+		return r, ErrDeclined
+	}
+	if res.status != C.AIGW_OK {
+		return r, nil
+	}
+	pl, bl := int(res.path_len), int(res.body_len)
+	if pl+bl > len(scratch) {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	copy(scratch, unsafe.Slice((*byte)(unsafe.Pointer(out.out)), int(out.out_used))[int(res.out_off):int(res.out_off)+pl+bl])
 	r.Path = scratch[:pl]
 	if !r.Unchanged {
 		r.Body = scratch[pl : pl+bl]
@@ -171,7 +222,8 @@ func CompletionsRequestSchema(backendSchema string) int {
 // RerankRequestSchema is the aigw_backend_cfg.schema of a Cohere /v2/rerank request to a backend of that schema (aigw_chat_translate_*
 // or the batcher: RerankEndpointSpec.ParseBody + RequestBody, endpointspec.go:364-383; api_version = the backend schema's Version), or
 // -1 when the backend has no translator for the endpoint (GetTranslator serves only Cohere) and the stock path reports that error.
-// The buffered response's usage comes from aigw_rerank_response_usage_host; rerank never streams.
+// The buffered response's usage comes from aigw_rerank_response_usage_host; rerank never streams.  Bodies above 65 536 bytes are
+// beyond the batcher's translate pass: TranslateRerank sends them to aigw_rerank_translate_large_host.
 func RerankRequestSchema(backendSchema string) int {
 	if backendSchema == "Cohere" {
 		return C.AIGW_SCHEMA_RERANK_COHERE
@@ -268,5 +320,6 @@ func (s *Stream) Close() { C.aigw_stream_close(s.p.ctx, s.h) }
 
 func (p *Pipeline) Close() {
 	C.aigw_batcher_stop(p.batcher)
+	C.aigw_destroy(p.bulk)
 	C.aigw_destroy(p.ctx)
 }
