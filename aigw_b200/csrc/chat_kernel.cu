@@ -24,35 +24,30 @@ namespace aigw {
 //   K2 walk    (thread per document)  stage 3+4 → jump table, copy ops, scratch, plan header
 //   K3 emit    (warp per document)    stage 5 → output record + result
 // K2 is where SIMT pays: 32 bodies with the same token count (≈ the same shape) share every instruction fetch.
-// Sub-batches are small enough for the bodies to stay in L2 between K1 and K3 (the body is read from DRAM once) and
-// alternate between two streams, so the latency-bound walk of one sub-batch runs under the issue-bound index / emit
-// of the other.
+// A call of several sub-batches runs K1 of sub-batch k+1 and K3 of sub-batch k in one paired launch (chat_pair_kernel,
+// launch_cls), so the issue-bound index and the bandwidth-bound emit share the SMs.
 // ---- K1: structural index, one warp per document
-template <int MAXD, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) chat_index_kernel(const __grid_constant__ ChatParams P, uint32_t doc0, uint32_t ndocs, uint8_t* work) {
+template <int MAXD>
+struct IndexSmem {
   using C = Cls<MAXD>;
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // CTA-shared tables: key/value id hash tables
-  IdTables* s_ids = (IdTables*)smem;
-  uint64_t* s_bar = (uint64_t*)(smem + sizeof(IdTables));
-  {
-    const uint32_t* src = (const uint32_t*)((P.schema & AIGW_SCHEMA_RERANK) ? &c_ids_rr : (P.schema & AIGW_SCHEMA_COMPLETIONS) ? &c_ids_cp : (P.schema & AIGW_SCHEMA_RESPONSES) ? &c_ids_rq : (P.schema & AIGW_SCHEMA_MESSAGES) ? &c_ids_msg : (P.schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK ? &c_ids_resp : &c_ids);
-    for (uint32_t i = threadIdx.x; i < sizeof(IdTables) / 4; i += blockDim.x) ((uint32_t*)s_ids)[i] = src[i];
-  }
-  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
-  __syncthreads();
-  constexpr int kHdr = (int)((sizeof(IdTables) + 8 * WARPS + 15) & ~(size_t)15);
-  constexpr int kNcBytes = ((MAXD / 1024 + 1) * 4 + 15) & ~15;   // one word per round: lanes (32-byte blocks) that hold a valid escape the encoder rewrites
-  constexpr int kWarpBytes = C::kIn + C::kTok * 6 + kNcBytes;
-  uint8_t* wb = smem + kHdr + (size_t)warp * kWarpBytes;
+  static constexpr int kNcBytes = ((MAXD / 1024 + 1) * 4 + 15) & ~15;   // one word per round: lanes (32-byte blocks) that hold a valid escape the encoder rewrites
+  static constexpr int kWarpBytes = C::kIn + C::kTok * 6 + kNcBytes;
+};
+
+// the key / value id tables of the request or response schema P.schema names
+__device__ __forceinline__ const IdTables* id_tables_of(int schema) {
+  return (schema & AIGW_SCHEMA_RERANK) ? &c_ids_rr : (schema & AIGW_SCHEMA_COMPLETIONS) ? &c_ids_cp : (schema & AIGW_SCHEMA_RESPONSES) ? &c_ids_rq : (schema & AIGW_SCHEMA_MESSAGES) ? &c_ids_msg : (schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK ? &c_ids_resp : &c_ids;
+}
+
+// The warp indexes documents of the sub-batch [doc0, doc0 + ndocs) (workspace wp) until the sub-batch's index counter runs out.
+// wb: the warp's shared memory (IndexSmem layout), bar / phase: the warp's mbarrier for the bulk copies.
+template <int MAXD>
+__device__ __forceinline__ void index_docs(const ChatParams& P, uint32_t doc0, uint32_t ndocs, const WorkPtrs& wp, uint8_t* wb, const IdTables* s_ids, uint64_t* bar, uint32_t& phase, int lane) {
+  using C = Cls<MAXD>;
   uint8_t* s_in = wb;
   uint32_t* s_tw = (uint32_t*)(wb + C::kIn);
   uint16_t* s_bs = (uint16_t*)(s_tw + C::kTok);   // running backslash count in front of each token; later overlaid by the lookup list
   uint32_t* s_nc = (uint32_t*)(wb + C::kIn + C::kTok * 6);
-  uint64_t* bar = &s_bar[warp];
-  const WorkPtrs wp = carve(work, ndocs, layout_of<MAXD>());
-  uint32_t phase = 0;
 
   // work fetch, one document ahead: the atomic and the location loads of document k+1 complete under the scan of document k
   uint32_t li = 0;
@@ -99,11 +94,31 @@ __global__ void __launch_bounds__(WARPS * 32) chat_index_kernel(const __grid_con
 #undef AIGW_NEXT_DOC
 }
 
+template <int MAXD, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) chat_index_kernel(const __grid_constant__ ChatParams P, uint32_t doc0, uint32_t ndocs, uint8_t* work) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // CTA-shared tables: key/value id hash tables
+  IdTables* s_ids = (IdTables*)smem;
+  uint64_t* s_bar = (uint64_t*)(smem + sizeof(IdTables));
+  {
+    const uint32_t* src = (const uint32_t*)id_tables_of(P.schema);
+    for (uint32_t i = threadIdx.x; i < sizeof(IdTables) / 4; i += blockDim.x) ((uint32_t*)s_ids)[i] = src[i];
+  }
+  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
+  __syncthreads();
+  constexpr int kHdr = (int)((sizeof(IdTables) + 8 * WARPS + 15) & ~(size_t)15);
+  uint32_t phase = 0;
+  index_docs<MAXD>(P, doc0, ndocs, carve(work, ndocs, layout_of<MAXD>()), smem + kHdr + (size_t)warp * IndexSmem<MAXD>::kWarpBytes, s_ids, &s_bar[warp], phase, lane);
+}
+
 // ---- Ks: counting sort by token count (documents with the same count almost always have the same shape).  Every block
-// scans the (tiny) histogram itself; positions inside a bin come from a global cursor.
+// scans the (tiny) histogram itself; positions inside a bin come from a global cursor.  Most documents of a corpus share a few
+// bins, so the lanes of a warp that hold the same bin take their positions with ONE atomic (match + rank): one atomic per
+// document serialised on those few cursors and made this kernel ~0.1 ms per 229 376 documents on an H100.
 __global__ void __launch_bounds__(1024) chat_sort_kernel(const uint32_t* ntok, const uint32_t* bins, uint32_t* cursor, uint32_t* perm, uint32_t ndocs) {
   __shared__ uint32_t s[kBins];
-  const int t = threadIdx.x;
+  const int t = threadIdx.x, lane = t & 31;
   const uint32_t v = bins[t];
   s[t] = v;
   __syncthreads();
@@ -112,9 +127,18 @@ __global__ void __launch_bounds__(1024) chat_sort_kernel(const uint32_t* ntok, c
   __syncthreads();
   s[t] = excl;
   __syncthreads();
-  for (uint32_t li = blockIdx.x * blockDim.x + t; li < ndocs; li += gridDim.x * blockDim.x) {
+  for (uint32_t l0 = blockIdx.x * blockDim.x; l0 < ndocs; l0 += gridDim.x * blockDim.x) {   // l0 is uniform: every warp runs every round
+    const uint32_t li = l0 + t;
+    const bool valid = li < ndocs;
+    const unsigned act = __ballot_sync(FULL, valid);
+    if (!valid) continue;
     const uint32_t b = bin_of(ntok[li]);
-    perm[s[b] + atomicAdd(&cursor[b], 1u)] = li;
+    const unsigned peers = __match_any_sync(act, b);
+    const int leader = __ffs(peers) - 1;
+    uint32_t base = 0;
+    if (lane == leader) base = atomicAdd(&cursor[b], (uint32_t)__popc(peers));
+    base = __shfl_sync(peers, base, leader);
+    perm[s[b] + base + __popc(peers & ((1u << lane) - 1u))] = li;
   }
 }
 
@@ -123,28 +147,18 @@ __global__ void __launch_bounds__(1024) chat_sort_kernel(const uint32_t* ntok, c
 // as 16-byte chunks, one chunk per lane: the op a chunk starts in comes from a scatter (last op starting at or before each
 // chunk) + running max scan instead of a search; chunks inside one op are a single funnel-shifted shared-memory read; the
 // chunks that straddle op boundaries are collected and assembled afterwards with every lane busy.
-template <int MAXD, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) chat_emit_kernel(const __grid_constant__ ChatParams P, uint32_t doc0, uint32_t ndocs, uint8_t* work) {
+// The warp emits documents of the sub-batch [doc0, doc0 + ndocs) (workspace wp) until the sub-batch's emit counter runs out.
+// wb: the warp's shared memory (EmitSmem layout), s_lits: the CTA's copy of the literal table.
+template <int MAXD>
+__device__ __forceinline__ void emit_docs(const ChatParams& P, uint32_t doc0, uint32_t ndocs, const WorkPtrs& wp, uint8_t* wb, const uint8_t* s_lits, uint64_t* bar, uint32_t& phase, int lane) {
   using C = Cls<MAXD>;
   using E = EmitSmem<MAXD>;
-  extern __shared__ __align__(128) uint8_t smem[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint8_t* s_lits = smem;
-  uint64_t* s_bar = (uint64_t*)(smem + sizeof(c_lits.bytes));
-  for (uint32_t i = threadIdx.x; i < sizeof(c_lits.bytes) / 4; i += blockDim.x) ((uint32_t*)s_lits)[i] = ((const uint32_t*)c_lits.bytes)[i];
-  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
-  __syncthreads();
-  constexpr int kHdr = (int)((sizeof(c_lits.bytes) + 8 * WARPS + 15) & ~(size_t)15);
-  uint8_t* wb = smem + kHdr + (size_t)warp * E::kWarpBytes;
   uint8_t* s_in = wb;
   uint32_t* s_pre = (uint32_t*)(wb + C::kIn);
   uint32_t* s_ops = s_pre + C::kOps + 4;
   uint8_t* s_scr = (uint8_t*)(s_ops + C::kOps);
   uint16_t* s_first = (uint16_t*)(s_scr + E::kScrB);
   uint32_t* s_bl = (uint32_t*)(s_first + kEmitTile);
-  uint64_t* bar = &s_bar[warp];
-  const WorkPtrs wp = carve(work, ndocs, layout_of<MAXD>());
-  uint32_t phase = 0;
 
   // work fetch, one document ahead: plan header, location and the first 32 ops of document k+1 are loaded under the emit of
   // document k (each of these loads used to stall the warp for a DRAM round trip at the top of the loop)
@@ -214,11 +228,62 @@ __global__ void __launch_bounds__(WARPS * 32) chat_emit_kernel(const __grid_cons
   }
 }
 
+template <int MAXD, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) chat_emit_kernel(const __grid_constant__ ChatParams P, uint32_t doc0, uint32_t ndocs, uint8_t* work) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint8_t* s_lits = smem;
+  uint64_t* s_bar = (uint64_t*)(smem + sizeof(c_lits.bytes));
+  for (uint32_t i = threadIdx.x; i < sizeof(c_lits.bytes) / 4; i += blockDim.x) ((uint32_t*)s_lits)[i] = ((const uint32_t*)c_lits.bytes)[i];
+  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
+  __syncthreads();
+  constexpr int kHdr = (int)((sizeof(c_lits.bytes) + 8 * WARPS + 15) & ~(size_t)15);
+  uint32_t phase = 0;
+  emit_docs<MAXD>(P, doc0, ndocs, carve(work, ndocs, layout_of<MAXD>()), smem + kHdr + (size_t)warp * EmitSmem<MAXD>::kWarpBytes, s_lits, &s_bar[warp], phase, lane);
+}
+
+// ---- K1 + K3 paired: the index of sub-batch k+1 and the emit of sub-batch k share the SMs in one launch.  Index is bound by issue
+// and shared-memory work and uses about a third of HBM bandwidth; emit is bound by HBM bandwidth.  There is no data dependency
+// between the two (separate workspace slots), so each CTA holds the header of both (id tables, literal table) and a per-warp
+// region that is the union of the two layouts (s_in at offset 0 in both).  Even warps start on the index list, odd warps on the
+// emit list; a warp that drains its list joins the other one, so both lists finish together.
+template <int MAXD>
+struct PairSmem { static constexpr int kWarpBytes = IndexSmem<MAXD>::kWarpBytes > EmitSmem<MAXD>::kWarpBytes ? IndexSmem<MAXD>::kWarpBytes : EmitSmem<MAXD>::kWarpBytes; };
+template <int WARPS>
+__host__ __device__ constexpr size_t pair_hdr_bytes() { return (sizeof(IdTables) + sizeof(LitTable::bytes) + 8 * WARPS + 15) & ~(size_t)15; }
+
+template <int MAXD, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) chat_pair_kernel(const __grid_constant__ ChatParams P, uint32_t doc0_idx, uint32_t n_idx, uint8_t* work_idx,
+                                                               uint32_t doc0_emit, uint32_t n_emit, uint8_t* work_emit) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  IdTables* s_ids = (IdTables*)smem;
+  uint8_t* s_lits = smem + sizeof(IdTables);
+  uint64_t* s_bar = (uint64_t*)(s_lits + sizeof(c_lits.bytes));
+  {
+    const uint32_t* src = (const uint32_t*)id_tables_of(P.schema);
+    for (uint32_t i = threadIdx.x; i < sizeof(IdTables) / 4; i += blockDim.x) ((uint32_t*)s_ids)[i] = src[i];
+    for (uint32_t i = threadIdx.x; i < sizeof(c_lits.bytes) / 4; i += blockDim.x) ((uint32_t*)s_lits)[i] = ((const uint32_t*)c_lits.bytes)[i];
+  }
+  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
+  __syncthreads();
+  uint8_t* wb = smem + pair_hdr_bytes<WARPS>() + (size_t)warp * PairSmem<MAXD>::kWarpBytes;
+  const WorkPtrs wi = carve(work_idx, n_idx, layout_of<MAXD>()), we = carve(work_emit, n_emit, layout_of<MAXD>());
+  uint32_t phase = 0;
+  if ((warp & 1) == 0) {
+    index_docs<MAXD>(P, doc0_idx, n_idx, wi, wb, s_ids, &s_bar[warp], phase, lane);
+    emit_docs<MAXD>(P, doc0_emit, n_emit, we, wb, s_lits, &s_bar[warp], phase, lane);
+  } else {
+    emit_docs<MAXD>(P, doc0_emit, n_emit, we, wb, s_lits, &s_bar[warp], phase, lane);
+    index_docs<MAXD>(P, doc0_idx, n_idx, wi, wb, s_ids, &s_bar[warp], phase, lane);
+  }
+}
+
 // ------------------------------------------------------------------ host-side launcher
 template <int MAXD>
 size_t work_bytes_cls(size_t ndocs) { return work_per_doc(layout_of<MAXD>()) * ndocs + kWorkHdr + 256; }
 
-struct ClsConfig { bool ready = false; int bps1 = 1, bps3 = 1; };
+struct ClsConfig { bool ready = false; int bps1 = 1, bps3 = 1, bpsp = 1; };
 
 // documents per sub-batch: the bodies of the sub-batches in flight (two streams) stay in the 50 MB L2 between index and emit
 static size_t sub_batch_docs(int maxd) {
@@ -229,13 +294,46 @@ static size_t sub_batch_docs(int maxd) {
   return p;
 }
 
+// Paired schedule (launch_cls): documents per sub-batch, at most; two workspace slots of this size must fit the 3 GiB workspace
+// cap (lib.cu ensure_chat_work), which a slot of more than ~236 000 documents at the 5120 class does not.  Every sub-batch adds a
+// walk launch with its own tail, and that costs more than the pairing saves at smaller sizes.  Measured on an H100 80GB HBM3 at
+// 700 W (SM 1980 MHz, no throttle), bench.py's config-2 call (1 M bodies of ~4 KB), paired vs the serial schedule in one process
+// (tools/bench_translate_schedule.py): 65 536: 14.57 vs 12.07 ms; 131 072: 11.84 vs 11.76 ms; 229 376: 11.62 vs 11.77 ms.
+// A call pairs only when it holds at least two full sub-batches of this size (kPairMinSubBatches; the workspace cap may then cut
+// the sub-batch of a large class smaller): below that the serial schedule runs it in one or two sub-batches of up to 262 144
+// documents.  The host call's chunks of ~1 KB bodies (bench.py config 5), paired at 131 072, were 7 % slower.  The call is
+// then cut into equal sub-batches of at most this size.  AIGW_CHAT_SUB overrides the size for measurements.
+static constexpr size_t kPairSubDocs = 229376;
+static constexpr size_t kPairMinSubBatches = 2;
+static size_t pair_sub_docs() {
+  static const long env = getenv("AIGW_CHAT_SUB") ? atol(getenv("AIGW_CHAT_SUB")) : 0;
+  return env > 0 ? (size_t)env : kPairSubDocs;
+}
+
+// Warps per CTA of the paired kernel, per class: as many resident warps per SM as the serial index and emit kernels have
+// (H100: 228 KB of shared memory per SM, 1 KB reserved per CTA; the CTA header is 8 448 bytes of tables + one mbarrier per warp):
+//   class   per-warp union   serial index / emit      paired
+//   2048     5 808 B          8 CTAs x 4 = 32 warps    4 CTAs x 8  = 32 warps    54 976 B per CTA
+//   5120    10 416 B          5 CTAs x 4 = 20          2 CTAs x 10 = 20         112 688 B
+//   9216    16 560 B          6 CTAs x 2 = 12          3 CTAs x 4  = 12          74 720 B
+//   17408   30 560 B          3 CTAs x 2 = 6           3 CTAs x 2  = 6           69 584 B
+// 0: the class keeps the serial schedule.  At 33792 and 65536 a CTA of the union layout holds a single warp and fewer CTAs fit
+// an SM than emit alone has (3 vs 4 and 1 vs 2), so pairing would cut emit's residency.
+constexpr int pair_warps(int maxd) { return maxd <= 2048 ? 8 : maxd <= 5120 ? 10 : maxd <= 9216 ? 4 : maxd <= 17408 ? 2 : 0; }
+static int class_of(uint32_t max_len) { return max_len <= 2048 ? 2048 : max_len <= 5120 ? 5120 : max_len <= 9216 ? 9216 : max_len <= 17408 ? 17408 : max_len <= 33792 ? 33792 : 65536; }
+// one slot of the paired schedule: `sub` documents' intermediates, 256-byte aligned
+static size_t pair_slot_bytes(int maxd, size_t sub) { return (chat_work_bytes((uint32_t)maxd, sub) + 255) & ~(size_t)255; }
+
 template <int MAXD, int WARPS>
 static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, const ChatAux* aux, cudaEvent_t* ev, int ev_cap,
                               int* launches) {
   using C = Cls<MAXD>;
+  constexpr int PW = pair_warps(MAXD) > 0 ? pair_warps(MAXD) : 1;   // PW is only used when pair_warps(MAXD) > 0
   constexpr size_t hdr1 = (sizeof(IdTables) + 8 * WARPS + 15) & ~(size_t)15, hdr3 = (sizeof(LitTable::bytes) + 8 * WARPS + 15) & ~(size_t)15;
-  const size_t smem1 = hdr1 + (size_t)(C::kIn + C::kTok * 6 + (((MAXD / 1024 + 1) * 4 + 15) & ~15)) * WARPS;
+  const size_t smem1 = hdr1 + (size_t)IndexSmem<MAXD>::kWarpBytes * WARPS;
   const size_t smem3 = hdr3 + (size_t)EmitSmem<MAXD>::kWarpBytes * WARPS;
+  constexpr size_t smemp = pair_hdr_bytes<PW>() + (size_t)PairSmem<MAXD>::kWarpBytes * PW;
+  static_assert(smemp <= 227 * 1024, "paired kernel's shared memory exceeds a CTA's limit");
   static ClsConfig cfgs[kMaxDevices];
   static std::mutex mu;
   if (device < 0 || device >= kMaxDevices) return cudaErrorInvalidDevice;
@@ -251,8 +349,15 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
       if (e != cudaSuccess) return e;
       e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bps3, chat_emit_kernel<MAXD, WARPS>, WARPS * 32, smem3);
       if (e != cudaSuccess) return e;
+      if constexpr (pair_warps(MAXD) > 0) {
+        e = cudaFuncSetAttribute(chat_pair_kernel<MAXD, PW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemp);
+        if (e != cudaSuccess) return e;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bpsp, chat_pair_kernel<MAXD, PW>, PW * 32, smemp);
+        if (e != cudaSuccess) return e;
+      }
       if (cc.bps1 < 1) cc.bps1 = 1;
       if (cc.bps3 < 1) cc.bps3 = 1;
+      if (cc.bpsp < 1) cc.bpsp = 1;
       cc.ready = true;
     }
   }
@@ -262,6 +367,46 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
   static const int env_emit_ctas = getenv("AIGW_EMIT_CTAS") ? atoi(getenv("AIGW_EMIT_CTAS")) : 0;
   static const int env_walk_ctas = getenv("AIGW_WALK_CTAS") ? atoi(getenv("AIGW_WALK_CTAS")) : 0;
   static const int env_pipe = getenv("AIGW_CHAT_PIPE") ? atoi(getenv("AIGW_CHAT_PIPE")) : 0;
+  // ---- paired schedule, two workspace slots (sub-batch k in slot k mod 2), one stream:
+  //   I(0) · S(0) W(0) · P(I(1)+E(0)) · S(1) W(1) · P(I(2)+E(1)) · … · S(n−1) W(n−1) · E(n−1)
+  // P is chat_pair_kernel: the index of the next sub-batch and the emit of this one share the SMs.  The walk runs alone (its
+  // registers make the register file the binding resource when it shares an SM).  Stage timing (ev) keeps the serial schedule
+  // below, whose four launches per sub-batch are what the stage split is read from.
+  if constexpr (pair_warps(MAXD) > 0) {
+    const size_t slot = (work_cap / 2) & ~(size_t)255;
+    size_t sub = slot > (size_t)kWorkHdr + 256 ? (slot - kWorkHdr - 256) / work_per_doc(layout_of<MAXD>()) : 0;
+    if (sub > pair_sub_docs()) sub = pair_sub_docs();
+    if (!ev && !env_pipe && env_streams <= 1 && sub > 0 && P.n >= kPairMinSubBatches * pair_sub_docs()) {
+      // equal sub-batches: a short last one would add a walk launch whose tail is as long as a full one's
+      const uint32_t nsb = (uint32_t)((P.n + sub - 1) / sub);
+      sub = (P.n + nsb - 1) / nsb;
+      auto nd_of = [&](uint32_t k) { return (uint32_t)((size_t)P.n - (size_t)k * sub < sub ? (size_t)P.n - (size_t)k * sub : sub); };
+      auto wk_of = [&](uint32_t k) { return work + (size_t)(k & 1u) * slot; };
+      auto grid = [&](long long units, int warps, int bps) { long long g = (long long)sm_count * bps, want = (units + warps - 1) / warps; return (unsigned)(want < g ? want : g); };
+      cudaError_t e;
+      if ((e = cudaMemsetAsync(wk_of(0), 0, kWorkHdr, st)) != cudaSuccess) return e;
+      chat_index_kernel<MAXD, WARPS><<<grid(nd_of(0), WARPS, cc.bps1), WARPS * 32, smem1, st>>>(P, first, nd_of(0), wk_of(0));
+      int nl = 1;
+      for (uint32_t k = 0; k < nsb; k++) {
+        const uint32_t nd = nd_of(k), doc0 = first + (uint32_t)(k * sub);
+        uint8_t* wk = wk_of(k);
+        const WorkPtrs wp = carve(wk, nd, layout_of<MAXD>());
+        { const unsigned gs = (nd + 8191) / 8192; chat_sort_kernel<<<gs < 32 ? gs : 32, kBins, 0, st>>>(wp.ntok, wp.bins, wp.cursor, wp.perm, nd); }
+        if ((e = launch_chat_walk(P, doc0, nd, wk, layout_of<MAXD>(), st, env_walk_ctas)) != cudaSuccess) return e;
+        if (k + 1 < nsb) {
+          // slot (k+1) mod 2 was last used by sub-batch k-1, whose emit ran in the previous paired launch
+          const uint32_t nn = nd_of(k + 1);
+          if ((e = cudaMemsetAsync(wk_of(k + 1), 0, kWorkHdr, st)) != cudaSuccess) return e;
+          chat_pair_kernel<MAXD, PW><<<grid((long long)nn + nd, PW, cc.bpsp), PW * 32, smemp, st>>>(P, doc0 + nd, nn, wk_of(k + 1), doc0, nd, wk);
+        } else {
+          chat_emit_kernel<MAXD, WARPS><<<grid(nd, WARPS, cc.bps3), WARPS * 32, smem3, st>>>(P, doc0, nd, wk);
+        }
+        nl += 3;
+      }
+      if (launches) *launches = nl;
+      return cudaGetLastError();
+    }
+  }
   // ---- stage-pipelined mode: one stream per STAGE, sub-batches flow index -> walk -> emit through a ring of workspaces, so in
   // the steady state one index, one walk and one emit kernel (of three consecutive sub-batches) are resident on every SM at
   // once.  The walk is latency-bound while index and emit are bound by the integer issue rate, so sharing an SM costs
@@ -362,19 +507,20 @@ size_t chat_work_bytes(uint32_t max_len, size_t ndocs) {
   if (max_len <= 33792) return work_bytes_cls<33792>(ndocs);
   return work_bytes_cls<65536>(ndocs);
 }
-// workspace that lets a call of n documents run at full overlap: two sub-batches in flight
+// workspace that lets a call of n documents run its schedule: two slots of the paired schedule, or two sub-batches in flight
+// in the experimental stream modes, or one sub-batch
 size_t chat_work_bytes_for(uint32_t max_len, size_t n) {
   static const int env_streams = getenv("AIGW_CHAT_STREAMS") ? atoi(getenv("AIGW_CHAT_STREAMS")) : 1;
   static const int env_pipe = getenv("AIGW_CHAT_PIPE") ? atoi(getenv("AIGW_CHAT_PIPE")) : 0;
-  if (env_pipe && n > 4096) {
-    const int maxd = max_len <= 2048 ? 2048 : max_len <= 5120 ? 5120 : max_len <= 9216 ? 9216 : max_len <= 17408 ? 17408 : max_len <= 33792 ? 33792 : 65536;
-    return kChatRing * ((chat_work_bytes(maxd, sub_batch_docs(maxd)) + 511) & ~(size_t)255) + 512;
+  const int maxd = class_of(max_len);
+  if (env_pipe && n > 4096) return kChatRing * ((chat_work_bytes(maxd, sub_batch_docs(maxd)) + 511) & ~(size_t)255) + 512;
+  if (n > 1024 && env_streams > 1) {
+    size_t sub = sub_batch_docs(maxd);
+    if (sub > n) sub = n;
+    return kChatStreams * (chat_work_bytes(max_len, sub) + 512);
   }
-  if (n <= 1024 || env_streams <= 1) return chat_work_bytes(max_len, n < 262144 ? n : 262144) + 512;
-  const int maxd = max_len <= 2048 ? 2048 : max_len <= 5120 ? 5120 : max_len <= 9216 ? 9216 : max_len <= 17408 ? 17408 : max_len <= 33792 ? 33792 : 65536;
-  size_t sub = sub_batch_docs(maxd);
-  if (sub > n) sub = n;
-  return kChatStreams * (chat_work_bytes(max_len, sub) + 512);
+  if (pair_warps(maxd) > 0 && n >= kPairMinSubBatches * pair_sub_docs()) return 2 * pair_slot_bytes(maxd, pair_sub_docs()) + 512;
+  return chat_work_bytes(max_len, n < 262144 ? n : 262144) + 512;
 }
 
 cudaError_t launch_chat_translate_range(const ChatParams& P, uint32_t first, uint32_t count, uint32_t max_len, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap,
