@@ -12,10 +12,10 @@ AIGW_WALK_DECL(0) AIGW_WALK_DECL(1) AIGW_WALK_DECL(2) AIGW_WALK_DECL(3) AIGW_WAL
 AIGW_SMALL_DECL(0) AIGW_SMALL_DECL(1) AIGW_SMALL_DECL(2) AIGW_SMALL_DECL(3) AIGW_SMALL_DECL(4) AIGW_SMALL_DECL(5) AIGW_SMALL_DECL(6) AIGW_SMALL_DECL(7) AIGW_SMALL_DECL(8) AIGW_SMALL_DECL(9) AIGW_SMALL_DECL(10) AIGW_SMALL_DECL(11) AIGW_SMALL_DECL(12)
 #undef AIGW_SMALL_DECL
 
-// resident walk blocks per SM.  The launch bound keeps room for AIGW_WALK_BLOCKS (the register budget), but the walk is bound by
-// L1 / L2 behaviour of its per-thread token lists and fewer warps run faster.  On an H100 80GB HBM3 at a 400 W power limit, walk
-// time per 1 M 4 KB bodies (bench.py config 2, the settings alternated within each of three runs of the bench): 4.13-4.17 ms at
-// 3 blocks over 9 runs, 4.35-4.37 ms at 4 blocks over 7 runs, 4.27-4.28 ms at 2 blocks over 2 runs.
+// resident walk blocks per SM.  The launch bound keeps room for AIGW_WALK_BLOCKS (the register budget: the Bedrock walk uses 116
+// registers), but fewer warps run faster.  On an H100 80GB HBM3 at a 700 W power limit (SM 1980 MHz, no throttle reason), profiled
+// walk time per 1 M 4 KB bodies (bench.py config 2, AIGW_WALK_CTAS, one session): 3.36-3.37 ms at 3 blocks over 3 runs, 3.38 ms at
+// 2 blocks, 3.54 ms at 4 blocks.
 constexpr int kWalkBlocksPerSm = 3;
 
 cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, const WorkLayout& layout, cudaStream_t st, int blocks_per_sm) {

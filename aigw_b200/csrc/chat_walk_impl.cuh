@@ -78,9 +78,12 @@ __device__ bool scalar_valid(const uint8_t* p, uint32_t n) {
 }
 
 // Stage 3: grammar check + bracket matching over the token list (single lane).  0 ok, else aigw_reason.
-__device__ int validate_tokens(Doc& d) {
-  const int MAXDEPTH = 48;
-  uint16_t open_idx[MAXDEPTH];
+// open_idx: kWalkDepth entries of local memory (Walker::stk).  Linking the stack through the jump table instead (a parent link
+// stored at the open bracket, read back at its close) made the Bedrock walk 2.7x slower on an H100: local memory is cached
+// write-back in L1, the global jump table is written through to L2.
+constexpr int kWalkDepth = 48;
+__device__ int validate_tokens(Doc& d, uint16_t* open_idx) {
+  const int MAXDEPTH = kWalkDepth;
   uint64_t isobj = 0;
   int depth = 0;
   // state: 0 value expected, 1 key or '}', 2 key, 3 ':', 4 ',' or close, 5 value or ']', 6 done
@@ -252,10 +255,15 @@ __device__ void emit_scalar_any(const Doc& d, Plan& pl, int vi, bool sys) {
   pl.src(d, o, l, sys);
 }
 
-__device__ void emit_any(const Doc& d, Plan& pl, int root, bool sys = false) {
-  const int MAXF = 24;
-  int f_open[MAXF]; int f_state[MAXF];  // array: current element token; object: last emitted key token (-1 none)
+// `stk` holds the open bracket of every container being emitted (kAnyDepth entries).  Only the innermost container's state
+// is kept in a register: a container with a child in progress is at that child (array: the element, which is the child's
+// open bracket; object: the key three tokens before it), so a pop recovers the parent's state from the child.
+constexpr int kAnyDepth = 24;
+static_assert(kAnyDepth <= kWalkDepth, "emit_any's stack is Walker::stk");
+__device__ void emit_any(const Doc& d, Plan& pl, uint16_t* stk, int root, bool sys = false) {
   int sp = 0;
+  int open = -1, state = 0;  // innermost container; array: current element token, object: last emitted key token (-1 none)
+  auto pop = [&]() { const int child = open; if (--sp) { open = stk[sp - 1]; state = d.ty(open) == '[' ? child : child - 3; } };
   int vi = root;
   bool need_value = true;
   for (;;) {
@@ -268,25 +276,24 @@ __device__ void emit_any(const Doc& d, Plan& pl, int root, bool sys = false) {
         pl.src(d, d.tok(vi), 1, sys);
         if (d.ty(vi + 1) == ']') pl.src(d, d.tok(vi + 1), 1, sys);
         else {
-          if (sp >= MAXF) { pl.err = AIGW_R_DEPTH; return; }
-          f_open[sp] = vi; f_state[sp] = vi + 1; sp++;
+          if (sp >= kAnyDepth) { pl.err = AIGW_R_DEPTH; return; }
+          stk[sp++] = (uint16_t)vi; open = vi; state = vi + 1;
           vi = vi + 1; need_value = true; continue;
         }
       } else if (c == '{') {
         pl.src(d, d.tok(vi), 1, sys);
-        if (sp >= MAXF) { pl.err = AIGW_R_DEPTH; return; }
-        f_open[sp] = vi; f_state[sp] = -1; sp++;
+        if (sp >= kAnyDepth) { pl.err = AIGW_R_DEPTH; return; }
+        stk[sp++] = (uint16_t)vi; open = vi; state = -1;
       } else emit_scalar_any(d, pl, vi, sys);
     }
     if (sp == 0) return;
-    const int open = f_open[sp - 1];
     if (d.ty(open) == '[') {
-      const int nx = d.next(f_state[sp - 1]);
+      const int nx = d.next(state);
       pl.src(d, d.tok(nx), 1, sys);  // ',' or ']'
-      if (d.ty(nx) == ',') { f_state[sp - 1] = nx + 1; vi = nx + 1; need_value = true; }
-      else sp--;
+      if (d.ty(nx) == ',') { state = nx + 1; vi = nx + 1; need_value = true; }
+      else pop();
     } else {
-      const int last = f_state[sp - 1];
+      const int last = state;
       int best = -1, cnt = 0;
       for (int m = open + 1; d.ty(m) != '}'; m = d.after(m + 3)) {
         if (d.str_has_backslash(m)) { pl.err = AIGW_R_ESCAPE; return; }
@@ -295,12 +302,12 @@ __device__ void emit_any(const Doc& d, Plan& pl, int root, bool sys = false) {
         if (c1 > 0 && (best < 0 || cmp_keys(d, m, best) < 0)) best = m;
         if (++cnt > 64) { pl.err = AIGW_R_UNSUPPORTED_FIELD; return; }
       }
-      if (best < 0) { pl.src(d, d.tok(d.jmp[open]), 1, sys); sp--; continue; }
+      if (best < 0) { pl.src(d, d.tok(d.jmp[open]), 1, sys); pop(); continue; }
       if (last >= 0) pl.lit(L_COMMA, sys);
       const uint32_t ko = d.tok(best), kc = d.tok(best + 1), colon = d.tok(best + 2);
       if (colon == kc + 1u) pl.src(d, ko, colon + 1u - ko, sys);
       else { pl.src(d, ko, kc + 1u - ko, sys); pl.lit(L_COLON, sys); }
-      f_state[sp - 1] = best;
+      state = best;
       vi = best + 3; need_value = true;
     }
   }
@@ -352,6 +359,7 @@ struct Walker {
   const ChatParams* P;
   int reason;
   int pending;  // first translator-side error (422 / internal): reported only if the rest of the body neither declines nor fails ParseBody
+  uint16_t* stk;  // walk_doc's only local array, for validate_tokens' open brackets and then emit_any's containers (never nested)
 
   __device__ __forceinline__ void decline(int r) { if (!reason) reason = r; }
   __device__ __forceinline__ void pend(int r) { if (!pending) pending = r; }
@@ -523,10 +531,10 @@ struct Walker {
   // (bedrockToolUseToOpenAICalls, internal/translator/openai_awsbedrock.go:623-641).  The marshalled text is planned
   // as ops first, then materialised into scratch with the escapes applied and replaced by one scratch op.
   __device__ void emit_escaped_json(int v) {
-    if (pl.dry) { emit_any(d, pl, v); return; }
+    if (pl.dry) { emit_any(d, pl, stk, v); return; }
     pl.flush();
     const int n0 = pl.nops; const uint32_t olen0 = pl.olen;
-    emit_any(d, pl, v);
+    emit_any(d, pl, stk, v);
     if (pl.err) return;
     pl.flush();
     const uint32_t start = sc.n;
@@ -583,7 +591,7 @@ struct Walker {
 
   // Buffered Bedrock Converse response → openai.ChatCompletionResponse (internal/translator/openai_awsbedrock.go:734-824).
   // terr: a known field has the wrong JSON type (the reference's decode fails: AIGW_INTERNAL); decline(): left to the stock path.
-  __device__ void plan_bedrock_response(uint32_t& path_len) {
+  __device__ __forceinline__ void plan_bedrock_response(uint32_t& path_len) {
     bool terr = false, unsup = false;
     if (is_null(0)) { decline(AIGW_R_UNSUPPORTED_FIELD); return; }      // zero struct: nil Output, the reference panics
     if (!is_obj(0)) { decline(AIGW_R_E500_DECODE); return; }
@@ -688,7 +696,7 @@ struct Walker {
           if (!bf) pl.lit(L_COMMA); bf = false;
           pl.lit(L_AM_TOOLUSE); if (t[2] >= 0) emit_str(t[2]); else pl.lit(L_EMPTY_STR);
           pl.lit(L_AN_NAME); if (t[0] >= 0) emit_str(t[0]); else pl.lit(L_EMPTY_STR);
-          pl.lit(L_TOOLUSE_INPUT); if (t[1] >= 0) emit_any(d, pl, t[1]); else pl.lit(L_NULL);
+          pl.lit(L_TOOLUSE_INPUT); if (t[1] >= 0) emit_any(d, pl, stk, t[1]); else pl.lit(L_NULL);
           if (bad()) return;
           pl.lit(L_RBRACE);
         } else if (q[2] >= 0) {
@@ -1176,7 +1184,7 @@ struct Walker {
     if (is_str(it.content)) emit_instance(it.content, task, title, first);
     else for (int q = it.content + 1; d.ty(q) != ']'; q = d.after(q)) emit_instance(is_null(q) ? -1 : q, task, title, first);
   }
-  __device__ void plan_embeddings(uint32_t& path_len, uint32_t& model_off, uint32_t& model_len, uint32_t& body_kind) {
+  __device__ __forceinline__ void plan_embeddings(uint32_t& path_len, uint32_t& model_off, uint32_t& model_len, uint32_t& body_kind) {
     const int base = P->schema & 15;
     body_kind = AIGW_BODY_UNCHANGED;
     int input = -1, model_raw = -1, model = -1, dims = -1, autot = -1, gtask = -1;
@@ -1355,11 +1363,11 @@ struct Walker {
     if (nt == 0 || nt == -AIGW_R_SYNTAX) { pend(AIGW_R_E500_ARGS); pl.lit(L_NULL); return; }
     if (nt < 0) { decline(-nt); return; }
     Doc a; a.s = sc.p; a.len = base + w; a.tw = tw_tail; a.jmp = jmp_tail; a.nt = nt; a.kind = 2;
-    { const int vr = validate_tokens(a); if (vr == AIGW_R_SYNTAX) { pend(AIGW_R_E500_ARGS); pl.lit(L_NULL); return; } if (vr) { decline(vr); return; } }
+    { const int vr = validate_tokens(a, stk); if (vr == AIGW_R_SYNTAX) { pend(AIGW_R_E500_ARGS); pl.lit(L_NULL); return; } if (vr) { decline(vr); return; } }
     const uint32_t c0 = a.ty(0);
     if (c0 == 'n') { pl.lit(L_NULL); return; }
     if (c0 != '{') { pend(AIGW_R_E500_ARGS); pl.lit(L_NULL); return; }  // not a map: "failed to unmarshal tool call arguments"
-    emit_any(a, pl, 0);
+    emit_any(a, pl, stk, 0);
   }
 
   // ---- Bedrock assistant content blocks (openai_awsbedrock.go:309-419)
@@ -1551,7 +1559,7 @@ struct Walker {
   }
 
   // ---- OpenAI → AWS Bedrock Converse (openai_awsbedrock.go:91-159)
-  __device__ void plan_bedrock(const Top& t, bool stream, uint32_t& path_len) {
+  __device__ __forceinline__ void plan_bedrock(const Top& t, bool stream, uint32_t& path_len) {
     emit_bedrock_path(t, stream);
     path_len = pl.olen;
     if (bad()) return;
@@ -1667,7 +1675,7 @@ struct Walker {
           pl.lit(L_TOOLSPEC_OPEN);
           if (ds >= 0 && d.str_len(ds) > 0) { pl.lit(L_DESC); emit_str(ds); pl.lit(L_COMMA); }
           pl.lit(L_INPUTSCHEMA);
-          if (pr >= 0) emit_any(d, pl, pr); else pl.lit(L_NULL);
+          if (pr >= 0) emit_any(d, pl, stk, pr); else pl.lit(L_NULL);
           if (bad()) return;
           pl.lit(L_NAME); if (nm >= 0) emit_str(nm); else pl.lit(L_EMPTY_STR); pl.lit(L_RBRACE);
           if (cache) pl.lit(L_TOOL_CACHE);
@@ -1689,14 +1697,20 @@ struct Walker {
     return true;
   }
 
+  // Validation of the OpenAI and Azure passthroughs, run once before either: the Bedrock walk with the plan in dry mode (its
+  // accept set ⊆ ParseBody's).  False when the body declines.
+  __device__ __forceinline__ bool passthrough_accepts(const Top& t, bool stream) {
+    { uint32_t pl0 = 0; pl.dry = true; plan_bedrock(t, stream, pl0); pl.dry = false; pl.nsys = 0; sc.n = 0; }
+    if (bad()) return false;
+    if (pending) { decline(AIGW_R_CONTENT); return false; }  // 422 / internal errors belong to the Bedrock translator; here the body is merely outside the fast path
+    return true;
+  }
+
   // ---- OpenAI → OpenAI passthrough (openai_openai.go:55-84) on top of ParseBody's forced include_usage
   // (endpointspec.go:107-123).  Edits follow tidwall/sjson `set`: an existing value is spliced in place, a missing key is
   // appended before the closing brace of the deepest existing object, and a rebuilt root loses the bytes outside its braces.
-  __device__ void plan_passthrough(const Top& t, bool stream, uint32_t& path_len, uint32_t& out_flags, uint32_t& body_kind) {
-    // validation = the Bedrock walk with the plan in dry mode (its accept set ⊆ ParseBody's)
-    { uint32_t pl0 = 0; pl.dry = true; plan_bedrock(t, stream, pl0); pl.dry = false; pl.nsys = 0; sc.n = 0; }
-    if (bad()) return;
-    if (pending) { decline(AIGW_R_CONTENT); return; }  // 422 / internal errors belong to the Bedrock translator; here the body is merely outside the fast path
+  // Runs after passthrough_accepts.
+  __device__ __forceinline__ void plan_passthrough(const Top& t, bool stream, uint32_t& path_len, uint32_t& out_flags, uint32_t& body_kind) {
     if (!emit_openai_path(path_len)) return;
     // which edits?
     bool inc_true = false; int iu_raw = -1;
@@ -2459,7 +2473,7 @@ struct Walker {
     const int ty = find(sch, MK_type), pr = find(sch, MK_properties), rq = find(sch, MK_required);
     pl.lit(L_MX_SCHEMA_TYPE);
     if (ty >= 0) emit_str(ty); else pl.lit(L_EMPTY_STR);
-    if (pr >= 0 && d.ty(pr + 1) != '}') { pl.lit(L_MX_PROPS); emit_any(d, pl, pr); }
+    if (pr >= 0 && d.ty(pr + 1) != '}') { pl.lit(L_MX_PROPS); emit_any(d, pl, stk, pr); }
     if (rq >= 0 && d.ty(rq + 1) != ']') {
       pl.lit(L_MX_REQUIRED);
       for (int e = rq + 1; d.ty(e) != ']'; e = d.after(e)) { if (e != rq + 1) pl.lit(L_COMMA); emit_str(e); }
@@ -2470,7 +2484,7 @@ struct Walker {
   __device__ void mx_str_array(int arr) { for (int e = arr + 1; d.ty(e) != ']'; e = d.after(e)) { if (e != arr + 1) pl.lit(L_COMMA); emit_str(e); } }
   __device__ void mx_max_tokens(const MxTop& t) { if (t.max_tokens >= 0) pl.src(d, d.tok(t.max_tokens), mx_plain_int(t.max_tokens)); else pl.lit(L_ZERO); }
 
-  __device__ void mx_openai(const MxTop& t, bool stream) {
+  __device__ __forceinline__ void mx_openai(const MxTop& t, bool stream) {
     // stop sequences: sjson marshals the []string with encoding/json; only spellings it shares with sonic are decided here
     if (t.stop >= 0) for (int e = t.stop + 1; d.ty(e) != ']'; e = d.after(e)) {
       if (d.str_nc(e)) { decline(AIGW_R_ESCAPE); return; }
@@ -2563,7 +2577,7 @@ struct Walker {
     if (ie >= 0 && d.ty(ie) == 't') pl.lit(L_MX_TR_STATUS_ERR); else pl.lit_tail(L_TOOLRESULT_MID, 1);
     emit_str(find(b, MK_tool_use_id)); pl.lit(L_TOOLRESULT_CLOSE);
   }
-  __device__ void mx_bedrock(const MxTop& t) {
+  __device__ __forceinline__ void mx_bedrock(const MxTop& t) {
     pl.lit(L_LBRACE);
     if (t.top_k >= 0) { pl.lit(L_MX_TOPK); pl.src(d, d.tok(t.top_k), d.scalar_end(t.top_k) - d.tok(t.top_k)); pl.lit(L_RBRACE); pl.lit(L_COMMA); }
     pl.lit(L_INF_OPEN); pl.lit(L_MAXTOK); mx_max_tokens(t);
@@ -2591,7 +2605,7 @@ struct Walker {
           else {
             pl.lit(L_TOOLUSE_OPEN); emit_str(find(b, MK_name)); pl.lit(L_TOOLUSE_INPUT);
             const int in = find(b, MK_input);
-            if (in >= 0) emit_any(d, pl, in); else pl.lit(L_NULL);
+            if (in >= 0) emit_any(d, pl, stk, in); else pl.lit(L_NULL);
             pl.lit(L_TOOLUSE_ID); emit_str(find(b, MK_id)); pl.lit(L_TOOLRESULT_CLOSE);
           }
         }
@@ -2656,11 +2670,8 @@ struct Walker {
   }
 
   // ---- OpenAI → Azure OpenAI (openai_azureopenai.go:37-62): the body is never rewritten; ":path" carries the deployment
-  // (= request model or the override, NOT path-escaped) and the api-version.
-  __device__ void plan_azure(const Top& t, bool stream, uint32_t& path_len, uint32_t& out_flags, uint32_t& body_kind) {
-    { uint32_t pl0 = 0; pl.dry = true; plan_bedrock(t, stream, pl0); pl.dry = false; pl.nsys = 0; sc.n = 0; }
-    if (bad()) return;
-    if (pending) { decline(AIGW_R_CONTENT); return; }
+  // (= request model or the override, NOT path-escaped) and the api-version.  Runs after passthrough_accepts.
+  __device__ __forceinline__ void plan_azure(const Top& t, bool stream, uint32_t& path_len, uint32_t& out_flags, uint32_t& body_kind) {
     if (stream && P->cost_configured) {  // ParseBody's forced include_usage still marks the request (endpointspec.go:107-123)
       int iu = -1;
       if (t.stream_options >= 0) iu = find(t.stream_options, K_include_usage);
@@ -2727,7 +2738,7 @@ struct Walker {
     if (nt == 0 || nt == -AIGW_R_SYNTAX) return false;
     if (nt < 0) { decline(-nt); return false; }
     Doc a; a.s = sc.p; a.len = base + w; a.tw = tw_tail; a.jmp = jmp_tail; a.nt = nt; a.kind = 2;
-    const int vr = validate_tokens(a);
+    const int vr = validate_tokens(a, stk);
     if (vr == AIGW_R_SYNTAX) return false;
     if (vr) { decline(vr); return false; }
     if (a.ty(0) != '{') return false;
@@ -2791,7 +2802,7 @@ struct Walker {
     if (!first) pl.lit(L_COMMA, sys); first = false;
     pl.lit(L_TEXT_OPEN, sys); emit_str(str_tok, sys); pl.lit(L_RBRACE, sys);
   }
-  __device__ void plan_gemini(const Top& t, bool stream, uint32_t& path_len) {
+  __device__ __forceinline__ void plan_gemini(const Top& t, bool stream, uint32_t& path_len) {
     { uint32_t pl0 = 0; pl.dry = true; plan_bedrock(t, stream, pl0); pl.dry = false; pl.nsys = 0; sc.n = 0; }
     if (bad()) return;
     pending = 0;   // Bedrock's translator errors do not apply
@@ -2877,10 +2888,10 @@ struct Walker {
         if (nm >= 0 && d.str_len(nm) > 0) { if (!f) pl.lit(L_COMMA); pl.lit(L_GEM_NAME); emit_str(nm); f = false; }
         if (pr >= 0) {
           const bool empty_obj = is_obj(pr) && d.ty(pr + 1) == '}';
-          if (json_schema) { if (!empty_obj) { if (!f) pl.lit(L_COMMA); pl.lit(L_GEM_PARAMS_JS); emit_any(d, pl, pr); } }
+          if (json_schema) { if (!empty_obj) { if (!f) pl.lit(L_COMMA); pl.lit(L_GEM_PARAMS_JS); emit_any(d, pl, stk, pr); } }
           else {
             if (!is_obj(pr)) { pend(AIGW_R_E422_CONTENT); }
-            else if (!empty_obj) { if (!gem_schema_ok(pr)) { decline(AIGW_R_UNSUPPORTED_FIELD); return; } if (!f) pl.lit(L_COMMA); pl.lit(L_GEM_PARAMS); emit_any(d, pl, pr); }
+            else if (!empty_obj) { if (!gem_schema_ok(pr)) { decline(AIGW_R_UNSUPPORTED_FIELD); return; } if (!f) pl.lit(L_COMMA); pl.lit(L_GEM_PARAMS); emit_any(d, pl, stk, pr); }
           }
           if (bad()) return;
         }
@@ -2922,7 +2933,7 @@ struct Walker {
   // ---- OpenAI → Anthropic messages API behind GCP rawPredict / AWS InvokeModel (anthropic_helper.go:455-569,661-747;
   // openai_gcpanthropic.go:56-100; openai_awsanthropic.go:54-100).  Only the layout the reference's goldens pin is
   // produced (testupstream_test.go:203,216,291,355,369,549); fields whose position the SDK decides are declined.
-  __device__ void plan_anthropic(const Top& t, bool stream, bool gcp, uint32_t& path_len) {
+  __device__ __forceinline__ void plan_anthropic(const Top& t, bool stream, bool gcp, uint32_t& path_len) {
     { uint32_t pl0 = 0; pl.dry = true; plan_bedrock(t, stream, pl0); pl.dry = false; pl.nsys = 0; sc.n = 0; }
     if (bad()) return;
     pending = 0;  // Bedrock's translator errors do not apply; this translator's own are found below
@@ -3113,6 +3124,7 @@ struct WalkBufs { const uint8_t* body; uint32_t len; uint32_t* tw; uint16_t* jmp
 // live in the global workspace (throughput path) or in shared memory (fused small-batch kernel).
 static __device__ __forceinline__ void walk_doc(const ChatParams& P, const WalkBufs B, uint32_t nt_word, PlanOut& po) {
   po.nops = 0; po.olen = 0; po.path_len = 0; po.model_off = 0; po.model_len = 0; po.flags = 0; po.reason = 0;
+  uint16_t stk[kWalkDepth];
   if constexpr (G == 8) {
     // error bodies: a body that is not JSON is still translated (it becomes the message), so an index-level failure is not final
     const bool idx_ok = !(nt_word & 0x80000000u);
@@ -3122,8 +3134,8 @@ static __device__ __forceinline__ void walk_doc(const ChatParams& P, const WalkB
     W.pl.ops = B.ops; W.pl.nops = 0; W.pl.nsys = 0; W.pl.cap = B.kOps; W.pl.clen = 0; W.pl.ckind = 0; W.pl.coff = 0; W.pl.olen = 0; W.pl.err = 0; W.pl.dry = false;
     W.sc.p = B.scr; W.sc.n = 0; W.sc.cap = (uint32_t)B.kScr - 20u;
     W.tw_tail = B.tw + nt8; W.jmp_tail = B.jmp + nt8; W.tail_cap = B.kTok - (int)nt8;
-    W.P = &P; W.reason = 0; W.pending = 0;
-    const bool tokens_ok = idx_ok && nt8 > 0 && validate_tokens(W.d) == 0;
+    W.P = &P; W.reason = 0; W.pending = 0; W.stk = stk;
+    const bool tokens_ok = idx_ok && nt8 > 0 && validate_tokens(W.d, stk) == 0;
     W.plan_response_error(tokens_ok);
     W.pl.flush();
     int reason = W.reason ? W.reason : W.pl.err;
@@ -3145,8 +3157,8 @@ static __device__ __forceinline__ void walk_doc(const ChatParams& P, const WalkB
   W.pl.ops = B.ops; W.pl.nops = 0; W.pl.nsys = 0; W.pl.cap = B.kOps; W.pl.clen = 0; W.pl.ckind = 0; W.pl.coff = 0; W.pl.olen = 0; W.pl.err = 0; W.pl.dry = false;
   W.sc.p = B.scr; W.sc.n = 0; W.sc.cap = (uint32_t)B.kScr - 20u;
   W.tw_tail = B.tw + ntok; W.jmp_tail = B.jmp + ntok; W.tail_cap = B.kTok - (int)ntok;
-  W.P = &P; W.reason = 0; W.pending = 0;
-  int reason = validate_tokens(W.d);
+  W.P = &P; W.reason = 0; W.pending = 0; W.stk = stk;
+  int reason = validate_tokens(W.d, stk);
   if (reason == AIGW_R_SYNTAX) reason = AIGW_R_E400_SYNTAX;
   uint32_t path_len = 0;
   if constexpr (G == 4 || G == 5) {
@@ -3203,9 +3215,10 @@ static __device__ __forceinline__ void walk_doc(const ChatParams& P, const WalkB
       po.flags = stream ? 1u : 0u;
       if constexpr (G == 0) W.plan_bedrock(t, stream, path_len);
       else if constexpr (G == 1) {
-        if (P.schema == AIGW_SCHEMA_OPENAI) { uint32_t fl = po.flags, bk = AIGW_BODY_BYTES; W.plan_passthrough(t, stream, path_len, fl, bk); po.flags = (uint8_t)(fl | (bk == AIGW_BODY_UNCHANGED ? 0x80u : 0u)); }
-        else if (P.schema == AIGW_SCHEMA_AZURE_OPENAI) { uint32_t fl = po.flags, bk = AIGW_BODY_UNCHANGED; W.plan_azure(t, stream, path_len, fl, bk); po.flags = (uint8_t)(fl | 0x80u); }
-        else W.decline(AIGW_R_SCHEMA);   // schemas without a planner land in this group
+        if (P.schema != AIGW_SCHEMA_OPENAI && P.schema != AIGW_SCHEMA_AZURE_OPENAI) W.decline(AIGW_R_SCHEMA);   // schemas without a planner land in this group
+        else if (!W.passthrough_accepts(t, stream)) {}
+        else if (P.schema == AIGW_SCHEMA_OPENAI) { uint32_t fl = po.flags, bk = AIGW_BODY_BYTES; W.plan_passthrough(t, stream, path_len, fl, bk); po.flags = (uint8_t)(fl | (bk == AIGW_BODY_UNCHANGED ? 0x80u : 0u)); }
+        else { uint32_t fl = po.flags, bk = AIGW_BODY_UNCHANGED; W.plan_azure(t, stream, path_len, fl, bk); po.flags = (uint8_t)(fl | 0x80u); }
       }
       else if constexpr (G == 2) W.plan_anthropic(t, stream, P.schema == AIGW_SCHEMA_GCP_ANTHROPIC, path_len);
       else if constexpr (G == 3) W.plan_gemini(t, stream, path_len);

@@ -15,7 +15,8 @@
 
 #ifndef AIGW_SF64_HD
 #ifdef __CUDACC__
-#define AIGW_SF64_HD __host__ __device__ __noinline__
+// inlined into the walk kernels: around an out-of-line call their live registers follow the call ABI, which costs spills
+#define AIGW_SF64_HD __host__ __device__ __attribute__((always_inline))
 #else
 #define AIGW_SF64_HD
 #endif
