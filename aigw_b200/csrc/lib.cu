@@ -118,7 +118,7 @@ struct aigw_ctx {
   struct StreamPool {
     std::mutex mu;
     Scratch<StreamSlot> d_slots; uint32_t cap = 0;   // cap: slots
-    std::vector<uint32_t> free_list, carry, gen, stamp; std::vector<uint8_t> open; uint32_t call_no = 0;
+    std::vector<uint32_t> free_list, carry, gen, stamp, kind, model_len; std::vector<uint8_t> open; uint32_t call_no = 0;   // kind, model_len: the slot's cfg (stream_out_cap)
     PinnedScratch<uint8_t> h_in; Scratch<uint8_t> d_in;
     PinnedScratch<StreamStep> h_steps; Scratch<StreamStep> d_steps;
     Scratch<aigw_chunk_result> d_res; PinnedScratch<aigw_chunk_result> h_res;
@@ -917,7 +917,7 @@ static int stream_pool_grow(aigw_ctx* ctx, uint32_t want) {
   CK(nd.ensure((size_t)ncap * sizeof(StreamSlot)));
   if (sp.cap) { CK(cudaMemcpyAsync(nd, sp.d_slots, (size_t)sp.cap * sizeof(StreamSlot), cudaMemcpyDeviceToDevice, ctx->s_compute)); CK(cudaStreamSynchronize(ctx->s_compute)); }
   sp.d_slots.swap(nd);
-  sp.carry.resize(ncap, 0); sp.gen.resize(ncap, 0); sp.stamp.resize(ncap, 0); sp.open.resize(ncap, 0);
+  sp.carry.resize(ncap, 0); sp.gen.resize(ncap, 0); sp.stamp.resize(ncap, 0); sp.open.resize(ncap, 0); sp.kind.resize(ncap, 0); sp.model_len.resize(ncap, 0);
   for (uint32_t i = ncap; i-- > sp.cap;) sp.free_list.push_back(i);
   sp.cap = ncap;
   return 0;
@@ -950,7 +950,7 @@ int aigw_stream_open_batch(aigw_ctx* ctx, const aigw_stream_cfg* cfg, uint32_t n
   CK(sp.h_ids.ensure((size_t)n * 4));
   for (uint32_t i = 0; i < n; i++) {
     const uint32_t slot = sp.free_list.back(); sp.free_list.pop_back();
-    sp.open[slot] = 1; sp.gen[slot]++; sp.carry[slot] = 0;
+    sp.open[slot] = 1; sp.gen[slot]++; sp.carry[slot] = 0; sp.kind[slot] = t->kind; sp.model_len[slot] = t->model_len;
     sp.h_ids[i] = slot; handles[i] = ((uint64_t)sp.gen[slot] << 32) | (uint64_t)(slot + 1);
   }
   cudaStream_t st = ctx->s_compute;
@@ -997,9 +997,7 @@ static int stream_chunks_core(aigw_ctx* ctx, uint32_t n, GET&& get, aigw_chunk_r
     s.slot = slot; s.len = c.len; s.eos = c.eos ? 1u : 0u;
     if (zc_base) s.in_off = (uint64_t)(c.bytes - zc_base);
     else { s.in_off = in_bytes; in_bytes += ((uint64_t)c.len + 15u) & ~15ull; }
-    // output bound: every unit of input (≥ 20 bytes) yields at most one chunk of ≤ 96 + id + model + its own text
-    const uint64_t oc = 16ull * ((uint64_t)sp.carry[slot] + c.len) + 1024u;
-    s.out_cap = (uint32_t)(oc > 0x7fffffffull ? 0x7fffffffull : oc);
+    s.out_cap = stream_out_cap(sp.kind[slot], (uint64_t)sp.carry[slot] + c.len, sp.model_len[slot]);
     s.out_off = out_bytes; out_bytes += ((uint64_t)s.out_cap + 15u) & ~15ull;
   }
   if (!zc_base) { CK(sp.h_in.ensure(in_bytes + 16)); CK(sp.d_in.ensure(in_bytes + 16)); }

@@ -128,12 +128,15 @@ __device__ void step_openai(StreamSlot& S, const StreamStep& st, uint8_t* out, a
       if (cp.obj_seen & (1u << C_OBJ_CTD)) { u.reasoning = cp.ints[C_REASONING]; u.mask |= 32u; }
     }
   }
-  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = AIGW_R_UNSUPPORTED_FIELD; return; }
-  S.beg = pos;
-  R.usage = u; R.body_kind = AIGW_BODY_UNCHANGED; R.out_len = 0;
   // responseModel = cmp.Or(streamingResponseModel, requestModel): placed after the (empty) body
   const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : completions ? 0u : S.model_len;
-  if (ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k]; R.model_len = ml; }
+  int reason = AIGW_R_UNSUPPORTED_FIELD;
+  if (!status && ml > st.out_cap) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; }
+  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = (uint32_t)reason; R.status = (uint8_t)status; R.reason = (uint8_t)reason; return; }
+  S.beg = pos;
+  R.usage = u; R.body_kind = AIGW_BODY_UNCHANGED; R.out_len = 0;
+  for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k];
+  R.model_len = ml;
 }
 
 // ------------------------------------------------------------------ S3: Anthropic SSE → OpenAI SSE
@@ -308,11 +311,13 @@ __device__ void step_anthropic(StreamSlot& S, const StreamStep& st, uint8_t* out
   }
   if (!status && st.eos && pos < n) { status = an_event(S, b + pos, n - pos, w); pos = n; }
   if (!status && st.eos) status = an_finish(S, w);
+  if (!status && w.n + S.model_len > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
   if (!status && w.ovf) status = AIGW_DECLINED;
   if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = w.ovf ? AIGW_R_OUT_SPACE : AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = (uint8_t)S.dead_reason; return; }
   S.beg = pos;
   R.usage = S.usage; R.out_len = w.n; R.body_kind = w.n ? AIGW_BODY_BYTES : AIGW_BODY_EMPTY;
-  if (w.n + S.model_len <= st.out_cap) { for (uint32_t k = 0; k < S.model_len; k++) out[w.n + k] = (uint8_t)S.model[k]; R.model_len = S.model_len; }
+  for (uint32_t k = 0; k < S.model_len; k++) out[w.n + k] = (uint8_t)S.model[k];
+  R.model_len = S.model_len;
 }
 
 // ------------------------------------------------------------------ S2: Bedrock eventstream → OpenAI SSE
@@ -430,10 +435,12 @@ __device__ void step_bedrock(StreamSlot& S, const StreamStep& st, uint8_t* out, 
     pos += total;
   }
   if (!status && st.eos) { if (wn + 13u > st.out_cap) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; } else { const char* dn = "data: [DONE]\n"; for (int k = 0; k < 13; k++) out[wn + k] = (uint8_t)dn[k]; wn += 13; } }
+  if (!status && wn + S.model_len > st.out_cap) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; }
   if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = (uint32_t)reason; R.status = (uint8_t)status; R.reason = (uint8_t)reason; return; }
   S.beg = pos;
   R.usage = u; R.out_len = wn; R.body_kind = wn ? AIGW_BODY_BYTES : AIGW_BODY_EMPTY;
-  if (wn + S.model_len <= st.out_cap) { for (uint32_t k = 0; k < S.model_len; k++) out[wn + k] = (uint8_t)S.model[k]; R.model_len = S.model_len; }
+  for (uint32_t k = 0; k < S.model_len; k++) out[wn + k] = (uint8_t)S.model[k];
+  R.model_len = S.model_len;
 }
 
 // ------------------------------------------------------------------ S3 behind AWS: Anthropic events wrapped in eventstream frames
@@ -549,11 +556,13 @@ __device__ void step_aws_anthropic(StreamSlot& S, const StreamStep& st, uint8_t*
     if (status) break;
   }
   if (!status && st.eos) status = an_finish(S, w);
+  if (!status && w.n + S.model_len > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
   if (!status && w.ovf) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; }
   if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = (uint32_t)reason; R.status = (uint8_t)status; R.reason = (uint8_t)reason; return; }
   S.beg = pos;
   R.usage = S.usage; R.out_len = w.n; R.body_kind = w.n ? AIGW_BODY_BYTES : AIGW_BODY_EMPTY;
-  if (w.n + S.model_len <= st.out_cap) { for (uint32_t k = 0; k < S.model_len; k++) out[w.n + k] = (uint8_t)S.model[k]; R.model_len = S.model_len; }
+  for (uint32_t k = 0; k < S.model_len; k++) out[w.n + k] = (uint8_t)S.model[k];
+  R.model_len = S.model_len;
 }
 
 // ------------------------------------------------------------------ S4 / R1: Gemini GenerateContentResponse → OpenAI
@@ -760,10 +769,12 @@ __device__ void step_gemini(StreamSlot& S, const StreamStep& st, uint8_t* out, a
     }
   }
   if (!status && st.eos) WL(w, "data: [DONE]\n");
+  if (!status && w.n + S.model_len > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
   if (!status && w.ovf) status = AIGW_DECLINED;
   if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = w.ovf ? AIGW_R_OUT_SPACE : AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = (uint8_t)S.dead_reason; return; }
   R.usage = u; R.out_len = w.n; R.body_kind = w.n ? AIGW_BODY_BYTES : AIGW_BODY_EMPTY;
-  if (w.n + S.model_len <= st.out_cap) { for (uint32_t k = 0; k < S.model_len; k++) out[w.n + k] = (uint8_t)S.model[k]; R.model_len = S.model_len; }
+  for (uint32_t k = 0; k < S.model_len; k++) out[w.n + k] = (uint8_t)S.model[k];
+  R.model_len = S.model_len;
 }
 
 // buffered response: the body accumulates in the slot; the last call (eos) converts it
@@ -797,12 +808,14 @@ __device__ void step_gemini_buffered(StreamSlot& S, const StreamStep& st, uint8_
     WL(w, ",\"object\":\"chat.completion\"");
     if (g.has_usage) { WL(w, ",\"usage\":"); gem_usage(w, g); }
     w.ch('}');
+    if (!status && w.n + ml > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
     if (w.ovf) status = AIGW_DECLINED;
     else {
       R.usage.input = g.prompt; R.usage.output = g.cand + g.thoughts; R.usage.total = g.total; R.usage.mask = 7u;
       if (g.has_usage) { R.usage.cached = g.cached; R.usage.reasoning = g.thoughts; R.usage.mask |= 8u | 32u; }
       R.out_len = w.n; R.body_kind = AIGW_BODY_BYTES;
-      if (w.n + ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[w.n + k] = m[k]; R.model_len = ml; }
+      for (uint32_t k = 0; k < ml; k++) out[w.n + k] = m[k];
+      R.model_len = ml;
       S.beg = S.end;
     }
   }
@@ -935,7 +948,10 @@ __device__ void step_anthropic_native(StreamSlot& S, const StreamStep& st, uint8
     if (!prefix(line, ll, "data: ", 6)) continue;
     if (native_event(S, line + 6, (int)ll - 6)) { status = AIGW_DECLINED; break; }
   }
-  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = AIGW_R_UNSUPPORTED_FIELD; return; }
+  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;
+  int reason = AIGW_R_UNSUPPORTED_FIELD;
+  if (!status && ml > st.out_cap) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; }
+  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = (uint32_t)reason; R.status = (uint8_t)status; R.reason = (uint8_t)reason; return; }
   {  // updateTotalTokens
     aigw_usage& u = S.usage;
     const bool out_set = u.mask & 2u;
@@ -945,8 +961,8 @@ __device__ void step_anthropic_native(StreamSlot& S, const StreamStep& st, uint8
   }
   S.beg = pos;
   R.usage = S.usage; R.body_kind = AIGW_BODY_UNCHANGED; R.out_len = 0;
-  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;
-  if (ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k]; R.model_len = ml; }
+  for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k];
+  R.model_len = ml;
 }
 
 // ------------------------------------------------------------------ S1 variant: /v1/responses, usage scan only
@@ -991,11 +1007,14 @@ __device__ void step_openai_responses(StreamSlot& S, const StreamStep& st, const
       u.cached = cp.ints[C_CACHED]; u.cache_creation = 0; u.reasoning = cp.ints[C_REASONING]; u.mask = 63u;
     }
   }
-  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = AIGW_R_UNSUPPORTED_FIELD; return; }
-  R.usage = u; R.body_kind = AIGW_BODY_UNCHANGED; R.out_len = 0;
   // responseModel = cmp.Or(streamingResponseModel, requestModel)
   const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;
-  if (ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k]; R.model_len = ml; }
+  int reason = AIGW_R_UNSUPPORTED_FIELD;
+  if (!status && ml > st.out_cap) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; }
+  if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = (uint32_t)reason; R.status = (uint8_t)status; R.reason = (uint8_t)reason; return; }
+  R.usage = u; R.body_kind = AIGW_BODY_UNCHANGED; R.out_len = 0;
+  for (uint32_t k = 0; k < ml; k++) out[k] = (uint8_t)m[k];
+  R.model_len = ml;
 }
 
 #include "stream_messages_openai.cuh"

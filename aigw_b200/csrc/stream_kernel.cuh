@@ -40,6 +40,34 @@ static_assert(sizeof(StreamSlot) == kStreamSlotBytes, "slot layout");
 
 struct StreamStep { uint32_t slot, len, eos, out_cap; uint64_t in_off, out_off; };   // 32 bytes
 
+// Output range of one call: the body the step writes, then the response model.  B = carry + chunk bytes the step decodes,
+// ml = the stream's request model length (≤ 160).  A unit is the smallest piece of input that yields output (a line, an SSE
+// event, an eventstream frame, a Gemini part); 16·B pays 16 bytes of output per input byte, so a kind needs more only where
+// one unit writes more than 16 bytes per byte it consumed:
+//   kind                        smallest unit with output                  most output of that unit             16·unit   extra per unit
+//   AWS Bedrock                 51 B: 16 B frame + 35 B metadata payload   ≤ 192 + id + model + role ≤ 576       816      0
+//   GCP Anthropic               30 B: "event: message_stop\ndata: {}\n\n"    ≤ 160 + id + model ≤ 480             480       0
+//   AWS Anthropic               60 B: frame of base64 {"type":"message_stop"}   the same ≤ 480                  960       0
+//   GCP Gemini                  4 B: "{}" + a 2-byte delimiter             66 + model (choices [])               64        2 + ml
+//   Gemini buffered             the whole body                              fixed text ≤ 500 + model             -         0
+//   /v1/messages, OpenAI        48 B: a data line with one text delta      ≤ 200 + its text                     768       0
+//   /v1/messages, OpenAI, buf.  3 B: one tool call "{}," in the body        49: {"type":"tool_use",…,"input":{}}  48        1
+//   /v1/messages, AWS Anthropic frame ≥ 16 B + its event JSON           the event JSON + ≤ 40                 -         0
+// (id, role and the text of a unit come from the input and are paid by 16·B except where they repeat in every unit: the Bedrock
+// id / model / role and the Anthropic message id, at most 160, 160, 64 and 160 bytes, are in the table.)  Once per call: 1024 for
+// one-time text (message_start, the end-of-stream chunk, [DONE], a last Gemini part without a delimiter) and the model.
+// The usage-only kinds (OpenAI, completions, native Anthropic, /v1/responses) write only the model: their bound stays 16·B + 1024.
+inline uint32_t stream_out_cap(uint32_t kind, uint64_t bytes, uint32_t model_len) {
+  uint64_t oc = 16ull * bytes + 1024u;
+  switch (kind) {
+    case AIGW_STREAM_OPENAI: case AIGW_STREAM_OPENAI_COMPLETIONS: case AIGW_STREAM_ANTHROPIC: case AIGW_STREAM_OPENAI_RESPONSES: break;
+    case AIGW_STREAM_GCP_GEMINI: oc += model_len + (bytes / 4 + 1) * (2ull + model_len); break;
+    case AIGW_STREAM_MESSAGES_OPENAI_BUFFERED: oc += model_len + bytes / 3 + 1; break;
+    default: oc += model_len; break;
+  }
+  return (uint32_t)(oc > 0x7fffffffull ? 0x7fffffffull : oc);
+}
+
 struct StreamParams {
   StreamSlot* slots;
   const uint8_t* in;             // the call's chunk bytes (device)

@@ -139,6 +139,8 @@ __device__ void step_messages_aws_anthropic(StreamSlot& S, const StreamStep& st,
     if (rc == 2) continue;
     WL(w, "event: "); w.raw(et, etl); WL(w, "\ndata: "); w.raw(t64, (uint32_t)dl); WL(w, "\n\n");
   }
+  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;
+  if (!status && w.n + ml > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
   if (!status && w.ovf) { status = AIGW_DECLINED; reason = AIGW_R_OUT_SPACE; }
   if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = (uint32_t)reason; R.status = (uint8_t)status; R.reason = (uint8_t)reason; return; }
   if (st.eos) {  // updateTotalTokens (anthropic_anthropic.go:176-201)
@@ -150,6 +152,6 @@ __device__ void step_messages_aws_anthropic(StreamSlot& S, const StreamStep& st,
   }
   S.beg = pos;
   R.usage = S.usage; R.out_len = w.n; R.body_kind = w.n ? AIGW_BODY_BYTES : AIGW_BODY_EMPTY;
-  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;
-  if (w.n + ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[w.n + k] = (uint8_t)m[k]; R.model_len = ml; }
+  for (uint32_t k = 0; k < ml; k++) out[w.n + k] = (uint8_t)m[k];
+  R.model_len = ml;
 }

@@ -173,12 +173,14 @@ __device__ void step_messages_openai(StreamSlot& S, const StreamStep& st, uint8_
     if (pos < n) { status = o2a_block(S, b + pos, n - pos, w); pos = n; }
     if (!status) o2a_closing(S, w);
   }
+  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;   // cmp.Or(state.model, requestModel)
+  if (!status && w.n + ml > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
   if (!status && w.ovf) status = AIGW_DECLINED;
   if (status) { S.flags |= SF_DEAD; S.dead_status = (uint32_t)status; S.dead_reason = w.ovf ? AIGW_R_OUT_SPACE : AIGW_R_UNSUPPORTED_FIELD; R.status = (uint8_t)status; R.reason = (uint8_t)S.dead_reason; return; }
   S.beg = pos;
   R.usage = S.usage; R.out_len = w.n; R.body_kind = w.n ? AIGW_BODY_BYTES : AIGW_BODY_EMPTY;
-  const char* m = S.rmodel_len ? S.rmodel : S.model; const uint32_t ml = S.rmodel_len ? S.rmodel_len : S.model_len;   // cmp.Or(state.model, requestModel)
-  if (w.n + ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[w.n + k] = (uint8_t)m[k]; R.model_len = ml; }
+  for (uint32_t k = 0; k < ml; k++) out[w.n + k] = (uint8_t)m[k];
+  R.model_len = ml;
 }
 
 // ---- buffered: the tool-call `arguments` string becomes the tool_use `input` object (json.Unmarshal into map[string]any, then
@@ -315,11 +317,13 @@ __device__ void step_messages_openai_buffered(StreamSlot& S, const StreamStep& s
     WL(w, ",\"model\":\""); w.raw(mp, ml); w.ch('"');
     if (stop) { WL(w, ",\"stop_reason\":\""); switch (stop) { case 2: WL(w, "max_tokens"); break; case 3: WL(w, "tool_use"); break; case 4: WL(w, "refusal"); break; default: WL(w, "end_turn"); break; } w.ch('"'); }
     WL(w, ",\"usage\":{\"cache_creation_input_tokens\":0,\"cache_read_input_tokens\":0,\"input_tokens\":"); w.dec(pt); WL(w, ",\"output_tokens\":"); w.dec(ct); WL(w, "}}");
+    if (!status && w.n + ml > st.out_cap) w.ovf = 1;   // the model follows the body in the same range
     if (!status && w.ovf) status = AIGW_DECLINED;
     if (!status) {
       R.usage.input = pt; R.usage.output = ct; R.usage.total = pt + ct; R.usage.mask = 7u;   // ExtractTokenUsageFromExplicitCaching(in, out, nil, nil)
       R.out_len = w.n; R.body_kind = AIGW_BODY_BYTES;
-      if (w.n + ml <= st.out_cap) { for (uint32_t k = 0; k < ml; k++) out[w.n + k] = mp[k]; R.model_len = ml; }
+      for (uint32_t k = 0; k < ml; k++) out[w.n + k] = mp[k];
+      R.model_len = ml;
       S.beg = S.end;
     }
   }

@@ -424,7 +424,8 @@ int aigw_bedrock_stream_host(aigw_ctx* ctx, const aigw_bedrock_stream_cfg* cfg, 
  * kind), followed by model_len bytes of responseModel; `usage` is the TokenUsage that call returns (the processor merges it
  * with Override); the arena stays valid until the next stream call on the context.  status: AIGW_OK; AIGW_INTERNAL = the
  * reference returns an error (stream failure); AIGW_DECLINED = outside the GPU path (reason: AIGW_R_UNSUPPORTED_FIELD,
- * AIGW_R_TOO_LARGE carry above 15.6 KB, AIGW_R_OUT_SPACE, AIGW_R_ARENA_FULL) — both are sticky for the stream.
+ * AIGW_R_TOO_LARGE carry above 15.6 KB, AIGW_R_OUT_SPACE = the call's body and model outgrew the output range the library sized
+ * for its kind (never expected for accepted input; the model is never dropped instead), AIGW_R_ARENA_FULL) — both are sticky for the stream.
  * cfg strings must not need JSON escaping (printable ASCII without '"' and '\\', ≤ 160 bytes), else -2. */
 enum aigw_stream_kind { AIGW_STREAM_OPENAI = 0, AIGW_STREAM_AWS_BEDROCK = 1, AIGW_STREAM_GCP_ANTHROPIC = 2, AIGW_STREAM_GCP_GEMINI = 3, AIGW_STREAM_GCP_GEMINI_BUFFERED = 4,
                         AIGW_STREAM_ANTHROPIC = 5, AIGW_STREAM_AWS_ANTHROPIC = 6, AIGW_STREAM_OPENAI_COMPLETIONS = 7,

@@ -3,6 +3,7 @@
 // on a CPU-only machine before it is run on the GPU.  Protocol on stdin, one command per line:
 //   open <kind> <request_model>            -> new slot
 //   feed <hex bytes> <eos 0|1>             -> prints: <status> <body_kind> <carry_len> <usage: in out total cached cc reasoning mask> <model hex> <body hex>
+//                                             <out_cap: the call's output range, stream_out_cap of lib.cu>
 // The append step of the real pipeline (stream_append_kernel) is restated in appendbytes() below.
 #define AIGW_HOST_HARNESS 1
 #include <cstdio>
@@ -37,20 +38,21 @@ int main() {
       std::vector<uint8_t> in = unhex(h);
       if (S->kind == AIGW_STREAM_OPENAI_RESPONSES) {   // no carry: stream_append_kernel leaves the slot alone, the step reads the call's bytes
         aigw_chunk_result R; memset(&R, 0, sizeof R);
-        StreamStep st{0, (uint32_t)in.size(), (uint32_t)eos, (uint32_t)(16 * in.size() + 1024), 0, 0};
+        StreamStep st{0, (uint32_t)in.size(), (uint32_t)eos, stream_out_cap(S->kind, in.size(), S->model_len), 0, 0};
         if (S->flags & SF_DEAD) R.status = (uint8_t)S->dead_status; else step_openai_responses(*S, st, in.data(), out.data(), R);
         printf("%d %d %u %u %u %u %u %u %u %u ", (int)R.status, (int)R.body_kind, S->end - S->beg, R.usage.input, R.usage.output, R.usage.total, R.usage.cached, R.usage.cache_creation, R.usage.reasoning, R.usage.mask);
-        hex(out.data() + R.out_len, R.model_len); printf(" "); hex(out.data(), R.out_len); printf("\n");
+        hex(out.data() + R.out_len, R.model_len); printf(" "); hex(out.data(), R.out_len); printf(" %u\n", st.out_cap);
         continue;
       }
       // stream_append_kernel: compact [beg, end) to the front, append the chunk
       const uint32_t keep = S->end - S->beg;
-      memmove(S->buf, S->buf + S->beg, keep); S->beg = 0; S->end = keep;
+      memmove(S->buf, S->buf + S->beg, keep); S->beg = 0; S->end = keep; S->_r0 = keep;
       aigw_chunk_result R; memset(&R, 0, sizeof R);
-      if (keep + in.size() > kStreamCarryCap) { printf("4 0 0 0 0 0 0 0 0 0 - -\n"); continue; }
+      const uint32_t out_cap = stream_out_cap(S->kind, keep + in.size(), S->model_len);
+      if (keep + in.size() > kStreamCarryCap) { printf("4 0 0 0 0 0 0 0 0 0 - - %u\n", out_cap); continue; }
       memcpy(S->buf + keep, in.data(), in.size()); S->end = keep + (uint32_t)in.size();
       memset(S->buf + S->end, 0, std::min<size_t>(16, kStreamCarryCap - S->end));
-      StreamStep st{0, (uint32_t)in.size(), (uint32_t)eos, (uint32_t)(16 * (keep + in.size()) + 1024), 0, 0};
+      StreamStep st{0, (uint32_t)in.size(), (uint32_t)eos, out_cap, 0, 0};
       if (S->flags & SF_DEAD) { R.status = (uint8_t)S->dead_status; }
       else switch (S->kind) {
         case AIGW_STREAM_OPENAI: step_openai(*S, st, out.data(), R); break;
@@ -68,7 +70,7 @@ int main() {
       }
       R.carry_len = S->end - S->beg;
       printf("%d %d %u %u %u %u %u %u %u %u ", (int)R.status, (int)R.body_kind, R.carry_len, R.usage.input, R.usage.output, R.usage.total, R.usage.cached, R.usage.cache_creation, R.usage.reasoning, R.usage.mask);
-      hex(out.data() + R.out_len, R.model_len); printf(" "); hex(out.data(), R.out_len); printf("\n");
+      hex(out.data() + R.out_len, R.model_len); printf(" "); hex(out.data(), R.out_len); printf(" %u\n", out_cap);
     }
   }
   return 0;
