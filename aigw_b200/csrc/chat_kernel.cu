@@ -285,15 +285,6 @@ size_t work_bytes_cls(size_t ndocs) { return work_per_doc(layout_of<MAXD>()) * n
 
 struct ClsConfig { bool ready = false; int bps1 = 1, bps3 = 1, bpsp = 1; };
 
-// documents per sub-batch: the bodies of the sub-batches in flight (two streams) stay in the 50 MB L2 between index and emit
-static size_t sub_batch_docs(int maxd) {
-  static const long env = getenv("AIGW_CHAT_SUB") ? atol(getenv("AIGW_CHAT_SUB")) : 0;
-  if (env > 0) return (size_t)env;
-  size_t d = ((size_t)20 << 20) / (size_t)maxd;
-  size_t p = 256; while (p * 2 <= d) p *= 2;
-  return p;
-}
-
 // Paired schedule (launch_cls): documents per sub-batch, at most; two workspace slots of this size must fit the 3 GiB workspace
 // cap (lib.cu ensure_chat_work), which a slot of more than ~236 000 documents at the 5120 class does not.  Every sub-batch adds a
 // walk launch with its own tail, and that costs more than the pairing saves at smaller sizes.  Measured on an H100 80GB HBM3 at
@@ -325,7 +316,7 @@ static int class_of(uint32_t max_len) { return max_len <= 2048 ? 2048 : max_len 
 static size_t pair_slot_bytes(int maxd, size_t sub) { return (chat_work_bytes((uint32_t)maxd, sub) + 255) & ~(size_t)255; }
 
 template <int MAXD, int WARPS>
-static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, const ChatAux* aux, cudaEvent_t* ev, int ev_cap,
+static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, cudaEvent_t* ev, int ev_cap,
                               int* launches) {
   using C = Cls<MAXD>;
   constexpr int PW = pair_warps(MAXD) > 0 ? pair_warps(MAXD) : 1;   // PW is only used when pair_warps(MAXD) > 0
@@ -361,12 +352,6 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
       cc.ready = true;
     }
   }
-  // stage timing (ev) needs the stages back to back on one stream; otherwise sub-batches rotate over the auxiliary streams
-  static const int env_streams = getenv("AIGW_CHAT_STREAMS") ? atoi(getenv("AIGW_CHAT_STREAMS")) : 1;   // > 1: sub-batches rotate over auxiliary streams
-  static const int env_idx_ctas = getenv("AIGW_IDX_CTAS") ? atoi(getenv("AIGW_IDX_CTAS")) : 0;      // experiments: cap resident CTAs per SM
-  static const int env_emit_ctas = getenv("AIGW_EMIT_CTAS") ? atoi(getenv("AIGW_EMIT_CTAS")) : 0;
-  static const int env_walk_ctas = getenv("AIGW_WALK_CTAS") ? atoi(getenv("AIGW_WALK_CTAS")) : 0;
-  static const int env_pipe = getenv("AIGW_CHAT_PIPE") ? atoi(getenv("AIGW_CHAT_PIPE")) : 0;
   // ---- paired schedule, two workspace slots (sub-batch k in slot k mod 2), one stream:
   //   I(0) · S(0) W(0) · P(I(1)+E(0)) · S(1) W(1) · P(I(2)+E(1)) · … · S(n−1) W(n−1) · E(n−1)
   // P is chat_pair_kernel: the index of the next sub-batch and the emit of this one share the SMs.  The walk runs alone (its
@@ -376,7 +361,7 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
     const size_t slot = (work_cap / 2) & ~(size_t)255;
     size_t sub = slot > (size_t)kWorkHdr + 256 ? (slot - kWorkHdr - 256) / work_per_doc(layout_of<MAXD>()) : 0;
     if (sub > pair_sub_docs()) sub = pair_sub_docs();
-    if (!ev && !env_pipe && env_streams <= 1 && sub > 0 && P.n >= kPairMinSubBatches * pair_sub_docs()) {
+    if (!ev && sub > 0 && P.n >= kPairMinSubBatches * pair_sub_docs()) {
       // equal sub-batches: a short last one would add a walk launch whose tail is as long as a full one's
       const uint32_t nsb = (uint32_t)((P.n + sub - 1) / sub);
       sub = (P.n + nsb - 1) / nsb;
@@ -392,7 +377,7 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
         uint8_t* wk = wk_of(k);
         const WorkPtrs wp = carve(wk, nd, layout_of<MAXD>());
         { const unsigned gs = (nd + 8191) / 8192; chat_sort_kernel<<<gs < 32 ? gs : 32, kBins, 0, st>>>(wp.ntok, wp.bins, wp.cursor, wp.perm, nd); }
-        if ((e = launch_chat_walk(P, doc0, nd, wk, layout_of<MAXD>(), st, env_walk_ctas)) != cudaSuccess) return e;
+        if ((e = launch_chat_walk(P, doc0, nd, wk, layout_of<MAXD>(), st, sm_count)) != cudaSuccess) return e;
         if (k + 1 < nsb) {
           // slot (k+1) mod 2 was last used by sub-batch k-1, whose emit ran in the previous paired launch
           const uint32_t nn = nd_of(k + 1);
@@ -407,93 +392,30 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
       return cudaGetLastError();
     }
   }
-  // ---- stage-pipelined mode: one stream per STAGE, sub-batches flow index -> walk -> emit through a ring of workspaces, so in
-  // the steady state one index, one walk and one emit kernel (of three consecutive sub-batches) are resident on every SM at
-  // once.  The walk is latency-bound while index and emit are bound by the integer issue rate, so sharing an SM costs
-  // each little; every kernel's grid is capped so that the three fit together (registers: 3x128x80 + 2x128x54 + 2x128x56).
-  if (env_pipe && aux && !ev && P.n > 4096) {
-    const int ic = env_idx_ctas > 0 ? env_idx_ctas : 2, wc = env_walk_ctas > 0 ? env_walk_ctas : 3, ec = env_emit_ctas > 0 ? env_emit_ctas : 2;
-    const int bps1 = ic < cc.bps1 ? ic : cc.bps1, bps3 = ec < cc.bps3 ? ec : cc.bps3;
-    size_t sub = sub_batch_docs(MAXD);
-    int ring = kChatRing;
-    const size_t per = (chat_work_bytes(MAXD, sub) + 511) & ~(size_t)255;
-    while (ring > 1 && per * ring > work_cap) ring--;
-    if (per * ring > work_cap) { sub = (work_cap - kWorkHdr - 256) / work_per_doc(layout_of<MAXD>()); ring = 1; }
-    if (sub == 0) return cudaErrorMemoryAllocation;
-    cudaStream_t sI = aux->s[0], sW = aux->s[1], sE = aux->s[2];
-    cudaError_t e;
-    if ((e = cudaEventRecord(aux->fork, st)) != cudaSuccess) return e;
-    if ((e = cudaStreamWaitEvent(sI, aux->fork, 0)) != cudaSuccess) return e;
-    int nl = 0, sb = 0;
-    for (uint32_t rel = 0; rel < P.n; rel += (uint32_t)sub, sb++) {
-      const uint32_t doc0 = first + rel;
-      const uint32_t nd = (uint32_t)(P.n - rel < sub ? P.n - rel : sub);
-      const int slot = sb % ring;
-      uint8_t* wk = work + (size_t)slot * per;
-      const WorkPtrs wp = carve(wk, nd, layout_of<MAXD>());
-      long long want = ((long long)nd + WARPS - 1) / WARPS;
-      long long g1 = (long long)sm_count * bps1; if (want < g1) g1 = want;
-      long long g3 = (long long)sm_count * bps3; if (want < g3) g3 = want;
-      if (sb >= ring && (e = cudaStreamWaitEvent(sI, aux->emit_done[slot], 0)) != cudaSuccess) return e;   // the slot's previous tenant has been emitted
-      if ((e = cudaMemsetAsync(wk, 0, kWorkHdr, sI)) != cudaSuccess) return e;
-      chat_index_kernel<MAXD, WARPS><<<(unsigned)g1, WARPS * 32, smem1, sI>>>(P, doc0, nd, wk);
-      if ((e = cudaEventRecord(aux->idx_done[slot], sI)) != cudaSuccess) return e;
-      if ((e = cudaStreamWaitEvent(sW, aux->idx_done[slot], 0)) != cudaSuccess) return e;
-      { const unsigned gs = (nd + 8191) / 8192; chat_sort_kernel<<<gs < 32 ? gs : 32, kBins, 0, sW>>>(wp.ntok, wp.bins, wp.cursor, wp.perm, nd); }
-      if ((e = launch_chat_walk(P, doc0, nd, wk, layout_of<MAXD>(), sW, wc)) != cudaSuccess) return e;
-      if ((e = cudaEventRecord(aux->walk_done[slot], sW)) != cudaSuccess) return e;
-      if ((e = cudaStreamWaitEvent(sE, aux->walk_done[slot], 0)) != cudaSuccess) return e;
-      chat_emit_kernel<MAXD, WARPS><<<(unsigned)g3, WARPS * 32, smem3, sE>>>(P, doc0, nd, wk);
-      if ((e = cudaEventRecord(aux->emit_done[slot], sE)) != cudaSuccess) return e;
-      nl += 4;
-    }
-    // emits complete in order on sE, and every index / walk precedes its emit
-    if ((e = cudaEventRecord(aux->join[0], sE)) != cudaSuccess) return e;
-    if ((e = cudaStreamWaitEvent(st, aux->join[0], 0)) != cudaSuccess) return e;
-    if (launches) *launches = nl;
-    return cudaGetLastError();
-  }
-  const bool overlap = aux && !ev && P.n > 1024 && env_streams > 1;
-  const int nstreams = overlap ? (env_streams < kChatStreams ? env_streams : kChatStreams) : 1;
-  const size_t half = (work_cap / nstreams) & ~(size_t)255;
-  size_t sub = (half - kWorkHdr - 256) / work_per_doc(layout_of<MAXD>());
-  const size_t want_sub = overlap ? sub_batch_docs(MAXD) : 262144;
-  if (sub > want_sub) sub = want_sub;
+  // ---- serial schedule, one stream, the whole workspace: index · sort · walk · emit per sub-batch of up to 262 144 documents
+  size_t sub = ((work_cap & ~(size_t)255) - kWorkHdr - 256) / work_per_doc(layout_of<MAXD>());
+  if (sub > 262144) sub = 262144;
   if (sub == 0) return cudaErrorMemoryAllocation;
   cudaError_t e;
-  if (overlap) {
-    if ((e = cudaEventRecord(aux->fork, st)) != cudaSuccess) return e;
-    for (int s = 0; s < nstreams; s++) if ((e = cudaStreamWaitEvent(aux->s[s], aux->fork, 0)) != cudaSuccess) return e;
-  }
-  const int bps1 = overlap && env_idx_ctas > 0 && env_idx_ctas < cc.bps1 ? env_idx_ctas : cc.bps1;
-  const int bps3 = overlap && env_emit_ctas > 0 && env_emit_ctas < cc.bps3 ? env_emit_ctas : cc.bps3;
   int nl = 0, sb = 0;
   for (uint32_t rel = 0; rel < P.n; rel += (uint32_t)sub, sb++) {
     const uint32_t doc0 = first + rel;
     const uint32_t nd = (uint32_t)(P.n - rel < sub ? P.n - rel : sub);
-    cudaStream_t s = overlap ? aux->s[sb % nstreams] : st;
-    uint8_t* wk = work + (size_t)(overlap ? (sb % nstreams) : 0) * half;
-    const WorkPtrs wp = carve(wk, nd, layout_of<MAXD>());
-    if ((e = cudaMemsetAsync(wk, 0, kWorkHdr, s)) != cudaSuccess) return e;
+    const WorkPtrs wp = carve(work, nd, layout_of<MAXD>());
+    if ((e = cudaMemsetAsync(work, 0, kWorkHdr, st)) != cudaSuccess) return e;
     long long want = ((long long)nd + WARPS - 1) / WARPS;
-    long long g1 = (long long)sm_count * bps1; if (want < g1) g1 = want;
-    long long g3 = (long long)sm_count * bps3; if (want < g3) g3 = want;
+    long long g1 = (long long)sm_count * cc.bps1; if (want < g1) g1 = want;
+    long long g3 = (long long)sm_count * cc.bps3; if (want < g3) g3 = want;
     const bool timed = ev && 4 * sb + 3 < ev_cap;
-    if (timed) cudaEventRecord(ev[4 * sb + 0], s);
-    chat_index_kernel<MAXD, WARPS><<<(unsigned)g1, WARPS * 32, smem1, s>>>(P, doc0, nd, wk);
-    if (timed) cudaEventRecord(ev[4 * sb + 1], s);
-    { const unsigned gs = (nd + 8191) / 8192; chat_sort_kernel<<<gs < 32 ? gs : 32, kBins, 0, s>>>(wp.ntok, wp.bins, wp.cursor, wp.perm, nd); }
-    if ((e = launch_chat_walk(P, doc0, nd, wk, layout_of<MAXD>(), s, env_walk_ctas)) != cudaSuccess) return e;
-    if (timed) cudaEventRecord(ev[4 * sb + 2], s);
-    chat_emit_kernel<MAXD, WARPS><<<(unsigned)g3, WARPS * 32, smem3, s>>>(P, doc0, nd, wk);
-    if (timed) cudaEventRecord(ev[4 * sb + 3], s);
+    if (timed) cudaEventRecord(ev[4 * sb + 0], st);
+    chat_index_kernel<MAXD, WARPS><<<(unsigned)g1, WARPS * 32, smem1, st>>>(P, doc0, nd, work);
+    if (timed) cudaEventRecord(ev[4 * sb + 1], st);
+    { const unsigned gs = (nd + 8191) / 8192; chat_sort_kernel<<<gs < 32 ? gs : 32, kBins, 0, st>>>(wp.ntok, wp.bins, wp.cursor, wp.perm, nd); }
+    if ((e = launch_chat_walk(P, doc0, nd, work, layout_of<MAXD>(), st, sm_count)) != cudaSuccess) return e;
+    if (timed) cudaEventRecord(ev[4 * sb + 2], st);
+    chat_emit_kernel<MAXD, WARPS><<<(unsigned)g3, WARPS * 32, smem3, st>>>(P, doc0, nd, work);
+    if (timed) cudaEventRecord(ev[4 * sb + 3], st);
     nl += 4;
-  }
-  if (overlap) {
-    for (int s = 0; s < nstreams; s++) {
-      if ((e = cudaEventRecord(aux->join[s], aux->s[s])) != cudaSuccess) return e;
-      if ((e = cudaStreamWaitEvent(st, aux->join[s], 0)) != cudaSuccess) return e;
-    }
   }
   if (launches) *launches = nl;
   return cudaGetLastError();
@@ -507,36 +429,21 @@ size_t chat_work_bytes(uint32_t max_len, size_t ndocs) {
   if (max_len <= 33792) return work_bytes_cls<33792>(ndocs);
   return work_bytes_cls<65536>(ndocs);
 }
-// workspace that lets a call of n documents run its schedule: two slots of the paired schedule, or two sub-batches in flight
-// in the experimental stream modes, or one sub-batch
+// workspace that lets a call of n documents run its schedule: two slots of the paired schedule, or one sub-batch
 size_t chat_work_bytes_for(uint32_t max_len, size_t n) {
-  static const int env_streams = getenv("AIGW_CHAT_STREAMS") ? atoi(getenv("AIGW_CHAT_STREAMS")) : 1;
-  static const int env_pipe = getenv("AIGW_CHAT_PIPE") ? atoi(getenv("AIGW_CHAT_PIPE")) : 0;
   const int maxd = class_of(max_len);
-  if (env_pipe && n > 4096) return kChatRing * ((chat_work_bytes(maxd, sub_batch_docs(maxd)) + 511) & ~(size_t)255) + 512;
-  if (n > 1024 && env_streams > 1) {
-    size_t sub = sub_batch_docs(maxd);
-    if (sub > n) sub = n;
-    return kChatStreams * (chat_work_bytes(max_len, sub) + 512);
-  }
   if (pair_warps(maxd) > 0 && n >= kPairMinSubBatches * pair_sub_docs()) return 2 * pair_slot_bytes(maxd, pair_sub_docs()) + 512;
   return chat_work_bytes(max_len, n < 262144 ? n : 262144) + 512;
 }
 
-cudaError_t launch_chat_translate_range(const ChatParams& P, uint32_t first, uint32_t count, uint32_t max_len, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap,
-                                        const ChatAux* aux, int* launches) {
-  ChatParams Q = P; Q.n = count;
-  return launch_chat_translate(Q, max_len, device, sm_count, st, work, work_cap, aux, launches, nullptr, 0, first);
-}
-
-cudaError_t launch_chat_translate(const ChatParams& P, uint32_t max_len, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, const ChatAux* aux, int* launches,
+cudaError_t launch_chat_translate(const ChatParams& P, uint32_t max_len, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, int* launches,
                                   cudaEvent_t* ev, int ev_cap, uint32_t first) {
-  if (max_len <= 2048) return launch_cls<2048, 4>(P, first, device, sm_count, st, work, work_cap, aux, ev, ev_cap, launches);
-  if (max_len <= 5120) return launch_cls<5120, 4>(P, first, device, sm_count, st, work, work_cap, aux, ev, ev_cap, launches);
-  if (max_len <= 9216) return launch_cls<9216, 2>(P, first, device, sm_count, st, work, work_cap, aux, ev, ev_cap, launches);
-  if (max_len <= 17408) return launch_cls<17408, 2>(P, first, device, sm_count, st, work, work_cap, aux, ev, ev_cap, launches);
-  if (max_len <= 33792) return launch_cls<33792, 1>(P, first, device, sm_count, st, work, work_cap, aux, ev, ev_cap, launches);
-  return launch_cls<65536, 1>(P, first, device, sm_count, st, work, work_cap, aux, ev, ev_cap, launches);
+  if (max_len <= 2048) return launch_cls<2048, 4>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 5120) return launch_cls<5120, 4>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 9216) return launch_cls<9216, 2>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 17408) return launch_cls<17408, 2>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 33792) return launch_cls<33792, 1>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  return launch_cls<65536, 1>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
 }
 
 }  // namespace aigw

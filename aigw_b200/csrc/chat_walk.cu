@@ -18,13 +18,9 @@ AIGW_SMALL_DECL(0) AIGW_SMALL_DECL(1) AIGW_SMALL_DECL(2) AIGW_SMALL_DECL(3) AIGW
 // 2 blocks, 3.54 ms at 4 blocks.
 constexpr int kWalkBlocksPerSm = 3;
 
-cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, const WorkLayout& layout, cudaStream_t st, int blocks_per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  { static int sm_cache[kMaxDevices] = {0}; if (dev >= 0 && dev < kMaxDevices) { if (!sm_cache[dev]) cudaDeviceGetAttribute(&sm_cache[dev], cudaDevAttrMultiProcessorCount, dev); sms = sm_cache[dev] ? sm_cache[dev] : 132; } }
+cudaError_t launch_chat_walk(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, const WorkLayout& layout, cudaStream_t st, int sm_count) {
   static const int env_ctas = getenv("AIGW_WALK_CTAS") ? atoi(getenv("AIGW_WALK_CTAS")) : 0;   // experiment: another number of resident blocks per SM
-  if (blocks_per_sm <= 0 || blocks_per_sm > AIGW_WALK_BLOCKS) blocks_per_sm = env_ctas > 0 && env_ctas <= AIGW_WALK_BLOCKS ? env_ctas : kWalkBlocksPerSm;
-  sms *= blocks_per_sm;
+  const int sms = sm_count * (env_ctas > 0 && env_ctas <= AIGW_WALK_BLOCKS ? env_ctas : kWalkBlocksPerSm);
   const uint32_t s = P.schema;
   if (s & (uint32_t)AIGW_SCHEMA_RERANK) return launch_chat_walk_g12(P, doc0, ndocs, work, layout, st, sms);   // declines every base but Cohere
   if (s & (uint32_t)AIGW_SCHEMA_COMPLETIONS) return launch_chat_walk_g11(P, doc0, ndocs, work, layout, st, sms);   // declines every base but OpenAI

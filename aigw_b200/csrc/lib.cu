@@ -82,7 +82,7 @@ struct ChunkSlot {
   Scratch<uint64_t> d_off; Scratch<uint32_t> d_len; Scratch<aigw_doc_result> d_res;
   Scratch<uint32_t> d_map;   // size-class bucketing: documents of the chunk grouped by class
   Scratch<uint8_t> d_out;
-  cudaEvent_t ev_h2d, ev_k0, ev_k1, ev_ctr, ev_done;
+  cudaEvent_t ev_h2d, ev_k1, ev_done;
 };
 
 struct aigw_bpe { Scratch<uint2> d_table; Scratch<uint16_t> d_b2i; uint32_t slots = 0; };
@@ -109,7 +109,6 @@ struct aigw_ctx {
   Scratch<unsigned long long> d_used_arr; PinnedScratch<unsigned long long> h_used_arr;  // per-chunk bump counters
   cudaEvent_t stage_ev[64]; float stage_ms[3] = {0, 0, 0}; int last_launches = 0;
   bool profile_stages = false;   // aigw_chat_set_profile: next device calls run the stages back to back on one stream and time them
-  ChatAux aux{};                 // two extra streams: sub-batches of one call alternate between them
   Scratch<uint8_t> d_stage[6];   // HostStage: one buffer per input table or output area of a single-shot host call (six at most)
   Scratch<uint8_t> d_bs_work;    // bedrock stream workspace (records + counts)
   PinnedScratch<uint8_t> h_chunk_res;   // chunk_pipeline: the mapped result table
@@ -391,15 +390,11 @@ int aigw_init(int device, aigw_ctx** out) {
   INIT_CK(cudaStreamCreateWithFlags(&ctx->s_compute, cudaStreamNonBlocking));
   INIT_CK(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
   INIT_CK(cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
-  for (int k = 0; k < kChatStreams; k++) { INIT_CK(cudaStreamCreateWithFlags(&ctx->aux.s[k], cudaStreamNonBlocking)); INIT_CK(cudaEventCreateWithFlags(&ctx->aux.join[k], cudaEventDisableTiming)); }
-  INIT_CK(cudaEventCreateWithFlags(&ctx->aux.fork, cudaEventDisableTiming));
-  for (int k = 0; k < kChatRing; k++) { INIT_CK(cudaEventCreateWithFlags(&ctx->aux.idx_done[k], cudaEventDisableTiming)); INIT_CK(cudaEventCreateWithFlags(&ctx->aux.walk_done[k], cudaEventDisableTiming)); INIT_CK(cudaEventCreateWithFlags(&ctx->aux.emit_done[k], cudaEventDisableTiming)); }
   INIT_CK(ctx->d_counters.ensure(256 * sizeof(unsigned int)));
   INIT_CK(cudaEventCreate(&ctx->ev0)); INIT_CK(cudaEventCreate(&ctx->ev1));
   for (auto& e2 : ctx->stage_ev) INIT_CK(cudaEventCreate(&e2));
   for (auto& s : ctx->slot) {
-    INIT_CK(cudaEventCreateWithFlags(&s.ev_h2d, cudaEventDisableTiming)); INIT_CK(cudaEventCreate(&s.ev_k0)); INIT_CK(cudaEventCreate(&s.ev_k1));
-    INIT_CK(cudaEventCreateWithFlags(&s.ev_ctr, cudaEventDisableTiming)); INIT_CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
+    INIT_CK(cudaEventCreateWithFlags(&s.ev_h2d, cudaEventDisableTiming)); INIT_CK(cudaEventCreate(&s.ev_k1)); INIT_CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
   }
 #undef INIT_CK
   *out = ctx;
@@ -411,14 +406,11 @@ void aigw_destroy(aigw_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   for (auto& s : ctx->slot) {
-    cudaEventDestroy(s.ev_h2d); cudaEventDestroy(s.ev_k0); cudaEventDestroy(s.ev_k1); cudaEventDestroy(s.ev_ctr); cudaEventDestroy(s.ev_done);
+    cudaEventDestroy(s.ev_h2d); cudaEventDestroy(s.ev_k1); cudaEventDestroy(s.ev_done);
   }
   for (auto& e2 : ctx->stage_ev) cudaEventDestroy(e2);
   cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1);
   cudaStreamDestroy(ctx->s_compute); cudaStreamDestroy(ctx->s_h2d); cudaStreamDestroy(ctx->s_d2h);
-  for (int k = 0; k < kChatStreams; k++) { if (ctx->aux.s[k]) cudaStreamDestroy(ctx->aux.s[k]); if (ctx->aux.join[k]) cudaEventDestroy(ctx->aux.join[k]); }
-  if (ctx->aux.fork) cudaEventDestroy(ctx->aux.fork);
-  for (int k = 0; k < kChatRing; k++) { if (ctx->aux.idx_done[k]) cudaEventDestroy(ctx->aux.idx_done[k]); if (ctx->aux.walk_done[k]) cudaEventDestroy(ctx->aux.walk_done[k]); if (ctx->aux.emit_done[k]) cudaEventDestroy(ctx->aux.emit_done[k]); }
   delete ctx;
 }
 
@@ -461,8 +453,8 @@ int aigw_memcpy_d2h(aigw_ctx* ctx, void* dst, const void* src, size_t bytes) { E
 int aigw_memset_d(aigw_ctx* ctx, void* dst, int v, size_t bytes) { ENTER(); CK(cudaMemset(dst, v, bytes)); return 0; }
 int aigw_sync(aigw_ctx* ctx) { ENTER(); CK(cudaDeviceSynchronize()); return 0; }
 
-// the translate workspace for `docs` documents planned at max_len bytes: two sub-batches in flight (one per auxiliary stream;
-// profiling runs one large sub-batch at a time), at most 3 GiB: the launcher walks a size class in sub-batches that fit it
+// the translate workspace for `docs` documents planned at max_len bytes: two sub-batch slots for a call the paired schedule
+// runs, one sub-batch otherwise, at most 3 GiB: the launcher walks a size class in sub-batches that fit it
 static int ensure_chat_work(aigw_ctx* ctx, uint32_t max_len, uint32_t docs) {
   size_t need = chat_work_bytes_for(max_len, docs);
   const size_t cap = (size_t)3 << 30, floor1 = chat_work_bytes(max_len, 1024);
@@ -483,7 +475,7 @@ static int chat_translate_device_impl(aigw_ctx* ctx, const aigw_backend_cfg* cfg
   const bool stages = ctx->profile_stages && kernel_ms;
   if (int rc = ensure_chat_work(ctx, ml, n)) return rc;
   if (int rc = timed(ctx, st, kernel_ms, [&] {
-        CK(launch_chat_translate(P, ml, ctx->device, ctx->sm_count, st, ctx->d_work, ctx->d_work.cap, &ctx->aux, &ctx->last_launches, stages ? ctx->stage_ev : nullptr, 64, first));
+        CK(launch_chat_translate(P, ml, ctx->device, ctx->sm_count, st, ctx->d_work, ctx->d_work.cap, &ctx->last_launches, stages ? ctx->stage_ev : nullptr, 64, first));
         return 0;
       }))
     return rc;
@@ -565,7 +557,6 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   //   SMs             index / sort / walk / emit of chunk c → device (s_compute)
   //   copy engine B   D2H of chunk c-1: exactly the bytes the emit stage produced + the chunk's result table (s_d2h)
   // The host runs one chunk behind the GPU (it waits for chunk c-1's byte count while chunk c's kernels are queued).
-  // AIGW_HOST_ZEROCOPY=1 restores the round-1 variant (emit stores straight into mapped host memory) for A/B runs.
   memset(out, 0, sizeof *out);
   if (n == 0) return 0;
   ENTER();
@@ -576,7 +567,6 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
       if (class_len(cfg, ml) <= kSmallMaxLen) return chat_small_host(ctx, cfg, bodies, offsets, lens, n, out);
     }
   }
-  static const bool zero_copy = getenv("AIGW_HOST_ZEROCOPY") != nullptr;
   static const uint64_t kChunkBytes = (uint64_t)(getenv("AIGW_CHUNK_MB") ? atol(getenv("AIGW_CHUNK_MB")) : 256) << 20;   // pipeline granularity (fill / drain cost vs per-chunk launches)
   const std::vector<uint32_t> cb = chunk_bounds(n, kChunkBytes, [&](uint32_t i) { return offsets[i]; }, [&](uint32_t i) { return offsets[i] + (((uint64_t)lens[i] + 15u) & ~15ull); });
   uint32_t max_len = 0;
@@ -597,7 +587,7 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   for (int s = 0; s < nslots; s++) {
     ChunkSlot& S = ctx->slot[s];
     CK(S.d_in.ensure(max_in + 64));
-    if (!zero_copy) CK(S.d_out.ensure(max_out + 64));
+    CK(S.d_out.ensure(max_out + 64));
     CK(S.d_off.ensure((size_t)max_docs * 8)); CK(S.d_len.ensure((size_t)max_docs * 4)); CK(S.d_res.ensure((size_t)max_docs * sizeof(aigw_doc_result)));
   }
   max_len = class_len(cfg, max_len);
@@ -608,8 +598,6 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
   CK(ctx->h_out.ensure(total_out_cap));
   CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result)));
   CK(ctx->d_used_arr.ensure((size_t)nch * 8)); CK(ctx->h_used_arr.ensure((size_t)nch * 8));
-  uint8_t* dev_out = nullptr; aigw_doc_result* dev_res = nullptr;  // device views of the pinned arenas (zero-copy variant)
-  if (zero_copy) { CK(cudaHostGetDevicePointer((void**)&dev_out, ctx->h_out, 0)); CK(cudaHostGetDevicePointer((void**)&dev_res, ctx->h_res, 0)); }
 
   ChatParams P0; fill_params(P0, cfg);
   uint64_t h2d = 0, d2h = (uint64_t)n * sizeof(aigw_doc_result) + (uint64_t)nch * 8;
@@ -620,12 +608,10 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     CK(cudaEventSynchronize(S.ev_k1));
     const uint64_t used = ctx->h_used_arr[k] < out_cap[k] ? ctx->h_used_arr[k] : out_cap[k];
     d2h += used;
-    if (!zero_copy) {
-      const uint32_t b = cb[k], nd = cb[k + 1] - b;
-      if (used) CK(cudaMemcpyAsync(ctx->h_out + out_base[k], S.d_out, used, cudaMemcpyDeviceToHost, ctx->s_d2h));
-      CK(cudaMemcpyAsync(ctx->h_res + b, S.d_res, (size_t)nd * sizeof(aigw_doc_result), cudaMemcpyDeviceToHost, ctx->s_d2h));
-      CK(cudaEventRecord(S.ev_done, ctx->s_d2h));
-    }
+    const uint32_t b = cb[k], nd = cb[k + 1] - b;
+    if (used) CK(cudaMemcpyAsync(ctx->h_out + out_base[k], S.d_out, used, cudaMemcpyDeviceToHost, ctx->s_d2h));
+    CK(cudaMemcpyAsync(ctx->h_res + b, S.d_res, (size_t)nd * sizeof(aigw_doc_result), cudaMemcpyDeviceToHost, ctx->s_d2h));
+    CK(cudaEventRecord(S.ev_done, ctx->s_d2h));
     return 0;
   };
   for (int c = 0; c < nch; c++) {
@@ -633,7 +619,7 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     const uint32_t b = cb[c], e = cb[c + 1], nd = e - b;
     if (c >= nslots) {
       CK(cudaStreamWaitEvent(ctx->s_h2d, S.ev_k1, 0));                       // the slot's input has been consumed
-      if (!zero_copy) CK(cudaStreamWaitEvent(ctx->s_compute, S.ev_done, 0));   // the slot's output has left the device
+      CK(cudaStreamWaitEvent(ctx->s_compute, S.ev_done, 0));                 // the slot's output has left the device
     }
     CK(cudaMemcpyAsync(S.d_in, bodies + offsets[b], in_bytes[c] - 16, cudaMemcpyHostToDevice, ctx->s_h2d));
     CK(cudaMemcpyAsync(S.d_off, offsets + b, (size_t)nd * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
@@ -661,17 +647,18 @@ int aigw_chat_translate_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const u
     // documents keep their global index: kernels address offsets/lens/results with doc0 + i (or doc_map[i]), and the absolute
     // offsets index straight into the chunk
     ChatParams P = P0;
-    chat_buffers(P, S.d_in - offsets[b], S.d_off - b, S.d_len - b, nd, zero_copy ? dev_out + out_base[c] : S.d_out, out_cap[c],
-                 zero_copy ? dev_res : S.d_res - b, ctx->d_used_arr + c, out_base[c], n_cls > 1 ? (const uint32_t*)S.d_map : nullptr);
+    chat_buffers(P, S.d_in - offsets[b], S.d_off - b, S.d_len - b, nd, S.d_out, out_cap[c], S.d_res - b, ctx->d_used_arr + c, out_base[c],
+                 n_cls > 1 ? (const uint32_t*)S.d_map : nullptr);
     if (n_cls <= 1) {
       int nl = 0;
-      CK(launch_chat_translate_range(P, b, nd, kClsMax[top_cls], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &ctx->aux, &nl));
+      CK(launch_chat_translate(P, kClsMax[top_cls], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &nl, nullptr, 0, b));
       out->gpu_launches += nl;
     } else {
       for (int k = 0; k < 6; k++) {
         if (!cls_cnt[k]) continue;
         int nl = 0;
-        CK(launch_chat_translate_range(P, cls_start[k], cls_cnt[k], kClsMax[k], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &ctx->aux, &nl));
+        P.n = cls_cnt[k];
+        CK(launch_chat_translate(P, kClsMax[k], ctx->device, ctx->sm_count, ctx->s_compute, ctx->d_work, ctx->d_work.cap, &nl, nullptr, 0, cls_start[k]));
         out->gpu_launches += nl;
       }
     }
