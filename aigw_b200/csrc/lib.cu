@@ -24,6 +24,7 @@
 #include "bpe_kernel.cuh"
 #include "emb_kernel.cuh"
 #include "rerank_large_kernel.cuh"
+#include "emb_large_kernel.cuh"
 
 #include <mutex>
 
@@ -103,6 +104,8 @@ struct aigw_ctx {
   Scratch<uint32_t> d_emb_tok; Scratch<uint64_t> d_emb_toff; Scratch<uint32_t> d_emb_tlen; Scratch<uint32_t> d_emb_cnt;
   // large rerank requests (aigw_rerank_translate_large_device): token and depth workspace, splice table
   Scratch<uint32_t> d_rr_tok; Scratch<uint8_t> d_rr_dep; Scratch<RerankSplice> d_rr_splice;
+  // large embeddings translations (aigw_embeddings_translate_large_device): one workspace slice per CTA (tokens, escapes, ops, scratch)
+  Scratch<uint8_t> d_el_ws;
   PinnedScratch<uint8_t> h_small;   // small-batch path: tables + bodies, read by the kernel in place
   // chat workspace (intermediates of one sub-batch) + per-stage timing events
   Scratch<uint8_t> d_work;
@@ -866,6 +869,118 @@ int aigw_rerank_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg,
   if (used) { CK(cudaMemcpyAsync(ctx->h_out, d_out, used, cudaMemcpyDeviceToHost, S.st)); CK(cudaStreamSynchronize(S.st)); }
   out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = S.h2d + 8; out->d2h_bytes = S.d2h + used;
   out->gpu_launches = 2; out->kernel_ms = ms;
+  return 0;
+}
+
+// ------------------------------------------------------------------ /v1/embeddings requests of any size below 16 MiB
+int aigw_embeddings_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                           const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                           aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  if (!ctx) return -2;
+  if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
+  ENTER_ON(stream);
+  ChatParams C;
+  fill_params(C, cfg);   // the ":path" prefix, override and api-version exactly as the translate pass gets them
+  const int32_t schema = cfg ? cfg->schema : -1;
+  const bool emb = schema == AIGW_SCHEMA_EMB_OPENAI || schema == AIGW_SCHEMA_EMB_AZURE_OPENAI || schema == AIGW_SCHEMA_EMB_GCP_VERTEX || schema == AIGW_SCHEMA_EMB_AWS_BEDROCK;
+  EmbLargeParams P;
+  P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.results = d_results;
+  P.out = d_out; P.out_capacity = out_capacity; P.out_used = (unsigned long long*)d_out_used;
+  P.call_reason = emb ? 0u : (uint32_t)AIGW_R_SCHEMA;
+  P.base = emb ? (uint32_t)(schema & 15) : 0u;
+  P.force_mutation = C.force_mutation ? 1u : 0u;
+  P.override_len = C.override_len;
+  P.override_ok = 1;
+  for (uint32_t i = 0; i < C.override_len; i++) { const uint32_t c = (uint8_t)C.override_model[i]; if (c < 0x20 || c > 0x7f || c == '"' || c == '\\') P.override_ok = 0; }
+  emb_large_lits(P, C.openai_path, C.prefix_len, C.override_model, C.override_len, C.api_version, C.version_len);
+  const uint32_t ml = max_len && max_len < (1u << 24) ? max_len : (1u << 24) - 1u;
+  P.tok_cap = emb_tok_cap(ml); P.esc_cap = emb_esc_cap(ml); P.op_cap = emb_op_cap(ml);
+  P.slice = emb_large_slice_bytes(ml);
+  const int grid = emb_large_grid(ctx->sm_count, ml);
+  CK(ctx->d_el_ws.ensure((size_t)grid * P.slice));
+  P.ws = ctx->d_el_ws;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_emb_large(P, grid, st)); return 0; });
+}
+
+int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                         const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  memset(out, 0, sizeof *out);
+  if (!ctx) return -2;
+  if (n == 0) return 0;
+  ENTER();
+  ChatParams C;
+  fill_params(C, cfg);
+  // output arena: Σ align16(path + 2 · len + 1024), the path bounded by the longest configuration path (or the model, at most the body)
+  const uint64_t path_max = (uint64_t)C.prefix_len + C.override_len + C.version_len + 64u;
+  uint32_t max_len = 0;
+  uint64_t cap = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (offsets[i] & 15u) { ctx->err = "aigw_embeddings_translate_large_host: request starts must be 16-byte aligned"; return -2; }
+    if (lens[i] > max_len) max_len = lens[i];
+    cap += (path_max + 2ull * lens[i] + 1024u + 15u) & ~15ull;
+  }
+  HostStage S(ctx);
+  const uint8_t* d_bodies = S.span(bodies, offsets, lens, n);
+  const uint64_t* d_off = S.in(offsets, n);
+  const uint32_t* d_len = S.in(lens, n);
+  uint8_t* d_out = S.out<uint8_t>(cap);
+  aigw_doc_result* d_res = S.out<aigw_doc_result>(n);
+  uint64_t* d_used = S.out<uint64_t>(1);
+  S.step([&] { CK(cudaMemsetAsync(d_used, 0, 8, S.st)); return 0; });
+  S.step([&] { CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result))); CK(ctx->h_used_arr.ensure(8)); return 0; });
+  if (S.rc) return S.rc;
+  float ms = 0;
+  if (int rc = aigw_embeddings_translate_large_device(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
+  S.back(ctx->h_res.p, d_res, n);
+  S.back((uint64_t*)ctx->h_used_arr.p, d_used, 1);
+  if (int rc = S.wait()) return rc;
+  uint64_t used = ctx->h_used_arr[0] < cap ? ctx->h_used_arr[0] : cap;
+  uint64_t h2d = S.h2d + 8, d2h = S.d2h;
+  uint32_t launches = 1;
+  // requests whose record did not fit report the length they need (body_len): run them once more into an arena of that size
+  std::vector<uint32_t> redo;
+  uint64_t cap2 = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    const aigw_doc_result& r = ctx->h_res[i];
+    if (r.status == AIGW_DECLINED && r.reason == AIGW_R_OUT_SPACE && r.body_len) { redo.push_back(i); cap2 += ((uint64_t)r.body_len + 15u) & ~15ull; }
+  }
+  // the host arena holds the first run's records, then the second run's
+  CK(ctx->h_out.ensure(used + cap2 + 16));
+  if (used) CK(cudaMemcpyAsync(ctx->h_out, d_out, used, cudaMemcpyDeviceToHost, S.st));
+  d2h += used;
+  if (!redo.empty()) {
+    // The retry stages into the first run's buffers (all but the bodies), and the first run's records are still being copied
+    // out of one of them: wait for that copy before anything may reallocate or overwrite it.
+    CK(cudaStreamSynchronize(S.st));
+    const uint32_t m = (uint32_t)redo.size();
+    std::vector<uint64_t> off2(m); std::vector<uint32_t> len2(m);
+    for (uint32_t k = 0; k < m; k++) { off2[k] = offsets[redo[k]]; len2[k] = lens[redo[k]]; }
+    HostStage S2(ctx);
+    S2.next = 1;   // the bodies stay staged in the first buffer; the others are free again (the first run and its copy are complete)
+    const uint64_t* d_off2 = S2.in(off2.data(), m);
+    const uint32_t* d_len2 = S2.in(len2.data(), m);
+    uint8_t* d_out2 = S2.out<uint8_t>(cap2);
+    aigw_doc_result* d_res2 = S2.out<aigw_doc_result>(m);
+    uint64_t* d_used2 = S2.out<uint64_t>(1);
+    S2.step([&] { CK(cudaMemsetAsync(d_used2, 0, 8, S2.st)); return 0; });
+    if (S2.rc) return S2.rc;
+    uint32_t ml2 = 0; for (uint32_t k = 0; k < m; k++) if (len2[k] > ml2) ml2 = len2[k];
+    float ms2 = 0;
+    if (int rc = aigw_embeddings_translate_large_device(ctx, cfg, d_bodies, d_off2, d_len2, m, ml2, d_out2, cap2, d_res2, d_used2, S2.st, &ms2)) return rc;
+    std::vector<aigw_doc_result> res2(m);
+    uint64_t used2 = 0;
+    S2.back(res2.data(), d_res2, m);
+    S2.back(&used2, d_used2, 1);
+    if (int rc = S2.wait()) return rc;
+    if (used2 > cap2) used2 = cap2;
+    if (used2) CK(cudaMemcpyAsync(ctx->h_out.p + used, d_out2, used2, cudaMemcpyDeviceToHost, S2.st));
+    CK(cudaStreamSynchronize(S2.st));
+    for (uint32_t k = 0; k < m; k++) { aigw_doc_result r = res2[k]; if (r.status == AIGW_OK) r.out_off += used; ctx->h_res[redo[k]] = r; }
+    h2d += S2.h2d + 8; d2h += S2.d2h + used2; used += used2; ms += ms2; launches++;
+  } else CK(cudaStreamSynchronize(S.st));
+  out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = h2d; out->d2h_bytes = d2h;
+  out->gpu_launches = launches; out->kernel_ms = ms;
   return 0;
 }
 

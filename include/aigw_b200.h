@@ -283,6 +283,41 @@ int aigw_rerank_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cf
 int aigw_rerank_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
                                      const uint32_t* lens, uint32_t n, aigw_batch_out* out);
 
+/* ---- /v1/embeddings requests of any size below 16 MiB ----
+ * The translate pass declines every AIGW_SCHEMA_EMB_* body above 64 KiB (AIGW_R_TOO_LARGE); a document-ingestion batch is larger.
+ * These calls stream one request through one CTA and give the results of aigw_chat_translate_* for the same schema and
+ * configuration (status, reason class, ":path", body_kind, body bytes, model span, flags 0; 400 / 422 / 500 in the same order),
+ * for bodies of 1 byte to 16 MiB - 1 (small ones included): the OpenAI / Azure passthrough with its model override splice, the
+ * GCP Vertex AI predict request and the Amazon Titan request, whose strings are re-encoded as the reference's encoder spells them
+ * (\/ -> /, \b \f -> \u0008 \u000c, \uXXXX -> UTF-8 with surrogate pairs joined, control characters as \n \r \t or \u00xx).
+ * Arguments, records and results are those of aigw_chat_translate_device / _host; `cfg->schema` other than AIGW_SCHEMA_EMB_OPENAI,
+ * _AZURE_OPENAI, _GCP_VERTEX, _AWS_BEDROCK declines every body with AIGW_R_SCHEMA.  Where they differ from the translate pass:
+ *   AIGW_R_ESCAPE      also a key with a backslash at the root or inside an input item (the translate pass compares decoded keys;
+ *                      clients do not escape "model" or "input"); a lone surrogate or bad hex in a re-encoded string, as there
+ *   AIGW_R_TOO_LARGE   a body of 16 MiB or more, a model above 65535 bytes, or a ":path" above 65535 bytes after PathEscape
+ *   AIGW_R_TOKENS      more than len / 2 + 1024 scan tokens (structural bytes outside strings, both quotes of every string, the
+ *                      first byte of every scalar; a token-id array costs two per id)
+ *   AIGW_R_DEPTH       nesting deeper than 48
+ *   AIGW_R_SCRATCH     (Vertex, Titan) more than len / 4 + 1024 escapes to re-spell (\/ \b \f \u): only strings made mostly of
+ *                      two-byte escapes reach it
+ *   AIGW_R_OPS         (Vertex) more than 2 * (len / 2 + 1024) copy ops: only input arrays made mostly of null elements, with a
+ *                      task type, reach it
+ *   AIGW_R_OUT_SPACE   a record longer than max(16 * len + 65536, 1048560) bytes (1048560: the translate pass's own record limit;
+ *                      body_len 0), such as a long request-level task_type repeated for many null inputs, whose record can pass
+ *                      4 GiB from a body of a few hundred KB; in the device form also a record that does not fit out_capacity,
+ *                      with body_len set to the record length (path and body) it needs.  Records are bump-allocated in the order
+ *                      requests finish.
+ * Workspace slices are sized by the call's longest body (max_len; 0 = unknown: sized for 16 MiB), so a call mixing one very large
+ * request with many small ones runs with few CTAs.  The host form is a staging wrapper around the device form: it sizes the
+ * output arena at align16(path + 2 * len + 1024) per body and sends the requests that still did not fit through the device form
+ * once more with the length each reported, so it never declines for output space.  `out` stays valid until the next
+ * host-buffer call on the context.  Offsets must be multiples of 16. */
+int aigw_embeddings_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                           const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                           aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                         const uint32_t* lens, uint32_t n, aigw_batch_out* out);
+
 /* ---- OpenAI SSE response streams: usage scan (S1) + TokenUsage merge (C1) ----
  * Stream s consists of chunks [chunk_first[s], chunk_first[s+1]); chunk c is bytes
  * [chunk_off[c], chunk_off[c+1]) of `bytes`.  For every stream the kernel replays the reference's

@@ -143,6 +143,47 @@ func (p *Pipeline) TranslateRerank(be Backend, cfg *C.aigw_backend_cfg, body, sc
 	return r, nil
 }
 
+// EmbeddingsBatcherMax is the largest /v1/embeddings body the batcher's translate pass holds; larger ones go to
+// aigw_embeddings_translate_large_host (TranslateEmbeddings).
+const EmbeddingsBatcherMax = 65536
+
+// TranslateEmbeddings is Translate for a backend registered with EmbeddingsRequestSchema: a body of up to EmbeddingsBatcherMax
+// bytes joins the backend's batch as before, a larger one (a document-ingestion batch, up to 16 MiB - 1) is streamed through one
+// CTA by aigw_embeddings_translate_large_host with the same semantics: the passthrough with its model override, the Vertex AI
+// predict request or the Titan request.  cfg is the configuration the backend was registered with.  The large call's record lives
+// in the context's pinned arena, so it is copied into scratch; a scratch smaller than the record declines.
+func (p *Pipeline) TranslateEmbeddings(be Backend, cfg *C.aigw_backend_cfg, body, scratch []byte) (Result, error) {
+	if len(body) <= EmbeddingsBatcherMax {
+		return p.Translate(be, body, scratch)
+	}
+	off, ln := C.uint64_t(0), C.uint32_t(len(body))
+	var out C.aigw_batch_out
+	p.bulkMu.Lock()
+	defer p.bulkMu.Unlock()
+	if rc := C.aigw_embeddings_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	res := *out.results
+	r := Result{Status: int(res.status), Reason: int(res.reason), Unchanged: res.body_kind == C.AIGW_BODY_UNCHANGED}
+	if res.status == C.AIGW_DECLINED {
+		return r, ErrDeclined
+	}
+	if res.status != C.AIGW_OK {
+		return r, nil
+	}
+	pl, bl := int(res.path_len), int(res.body_len)
+	if pl+bl > len(scratch) {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	copy(scratch, unsafe.Slice((*byte)(unsafe.Pointer(out.out)), int(out.out_used))[int(res.out_off):int(res.out_off)+pl+bl])
+	r.Path = scratch[:pl]
+	if !r.Unchanged {
+		r.Body = scratch[pl : pl+bl]
+	}
+	r.Model = body[int(res.model_off) : int(res.model_off)+int(res.model_len)]
+	return r, nil
+}
+
 // ---- response streams: Translator.ResponseBody(hdrs, body, endOfStream), one call per upstream chunk -------------------
 
 // Stream is one response stream's device-resident state (parser state + the undecoded tail of the bytes fed so far).
@@ -227,6 +268,24 @@ func CompletionsRequestSchema(backendSchema string) int {
 func RerankRequestSchema(backendSchema string) int {
 	if backendSchema == "Cohere" {
 		return C.AIGW_SCHEMA_RERANK_COHERE
+	}
+	return -1
+}
+
+// EmbeddingsRequestSchema is the aigw_backend_cfg.schema of a /v1/embeddings request to a backend of that schema
+// (EmbeddingsEndpointSpec.GetTranslator, endpointspec.go:243-256: OpenAI, AzureOpenAI, GCPVertexAI, AWSBedrock), or -1 when the
+// backend has no translator for the endpoint and the stock path reports that error.  Bodies above 65 536 bytes are beyond the
+// batcher's translate pass: TranslateEmbeddings sends them to aigw_embeddings_translate_large_host.
+func EmbeddingsRequestSchema(backendSchema string) int {
+	switch backendSchema {
+	case "OpenAI":
+		return C.AIGW_SCHEMA_EMB_OPENAI
+	case "AzureOpenAI":
+		return C.AIGW_SCHEMA_EMB_AZURE_OPENAI
+	case "GCPVertexAI":
+		return C.AIGW_SCHEMA_EMB_GCP_VERTEX
+	case "AWSBedrock":
+		return C.AIGW_SCHEMA_EMB_AWS_BEDROCK
 	}
 	return -1
 }
