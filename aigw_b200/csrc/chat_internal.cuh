@@ -264,15 +264,20 @@ constexpr IdTables make_rr_id_tables() {
 static_assert(id_max_probe(make_rr_id_tables().key, kKeySlots) <= 6, "rerank id hash table needs more than 6 probes");
 static __device__ __constant__ IdTables c_ids_rr = make_rr_id_tables();
 
-// id of a short string (1 ≤ n ≤ kMaxIdLen) held in shared memory, against the key or the value table (also in shared
-// memory).  Straight-line code: seven aligned word loads, funnel shifts, length mask, multiplicative hash, ≤ 4 probes.
+// id of a short string (1 ≤ n ≤ kMaxIdLen) held in shared memory (GLOBAL: in global memory), against the key or the value table
+// (in shared memory).  Straight-line code: eight aligned word loads, funnel shifts, length mask, multiplicative hash, ≤ 4 probes.
+// From global memory only the words that hold a byte of p[0, n) are read, so a string at the end of an allocation stays inside it.
+template <bool GLOBAL>
 __device__ __forceinline__ uint32_t lookup_id(const IdTables* T, const uint8_t* p, uint32_t n, bool key) {
-  const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
+  const uint32_t a = GLOBAL ? (uint32_t)(uintptr_t)p : (uint32_t)__cvta_generic_to_shared(p);
   const uint32_t sh = (a & 3u) * 8u;
   const uint32_t* wp = (const uint32_t*)(p - (a & 3u));
   uint32_t x[kIdWords + 1];
 #pragma unroll
-  for (int k = 0; k < kIdWords + 1; k++) x[k] = wp[k];
+  for (int k = 0; k < kIdWords + 1; k++) {
+    if constexpr (GLOBAL) x[k] = k == 0 || 4u * k < (a & 3u) + n ? __ldg(wp + k) : 0u;
+    else x[k] = wp[k];
+  }
   uint32_t v[kIdWords];
 #pragma unroll
   for (int k = 0; k < kIdWords; k++) {

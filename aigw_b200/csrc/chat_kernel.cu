@@ -3,7 +3,9 @@
 //
 //   * tokens carry their byte (tty) and a precomputed key / value id (tkid) that 32 lanes compute in
 //     parallel, so the schema walk compares one byte instead of strings;
-//   * request bodies are staged into shared memory by 1-D bulk asynchronous copies (bulk.cuh);
+//   * the index stage reads request bodies straight from global memory (the next body is prefetched into L2),
+//     so a warp's shared memory holds only its token words; the emit stage stages the body into shared memory
+//     by a 1-D bulk asynchronous copy (bulk.cuh) that overlaps the loading of its ops;
 //   * the output record is assembled as 16-byte chunks (one chunk per lane, funnel-shifted unaligned
 //     reads from shared memory) and stored straight to the arena — no shared-memory image of the output.
 #include "chat_internal.cuh"
@@ -25,13 +27,13 @@ namespace aigw {
 //   K3 emit    (warp per document)    stage 5 → output record + result
 // K2 is where SIMT pays: 32 bodies with the same token count (≈ the same shape) share every instruction fetch.
 // A call of several sub-batches runs K1 of sub-batch k+1 and K3 of sub-batch k in one paired launch (chat_pair_kernel,
-// launch_cls), so the issue-bound index and the bandwidth-bound emit share the SMs.
+// launch_cls), so the two stages, both latency-bound at the residency their shared memory allows (DESIGN.md §4.1), share the SMs.
 // ---- K1: structural index, one warp per document
 template <int MAXD>
 struct IndexSmem {
   using C = Cls<MAXD>;
   static constexpr int kNcBytes = ((MAXD / 1024 + 1) * 4 + 15) & ~15;   // one word per round: lanes (32-byte blocks) that hold a valid escape the encoder rewrites
-  static constexpr int kWarpBytes = C::kIn + C::kTok * 6 + kNcBytes;
+  static constexpr int kWarpBytes = C::kTok * 6 + kNcBytes;
 };
 
 // the key / value id tables of the request or response schema P.schema names
@@ -39,15 +41,15 @@ __device__ __forceinline__ const IdTables* id_tables_of(int schema) {
   return (schema & AIGW_SCHEMA_RERANK) ? &c_ids_rr : (schema & AIGW_SCHEMA_COMPLETIONS) ? &c_ids_cp : (schema & AIGW_SCHEMA_RESPONSES) ? &c_ids_rq : (schema & AIGW_SCHEMA_MESSAGES) ? &c_ids_msg : (schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK ? &c_ids_resp : &c_ids;
 }
 
-// The warp indexes documents of the sub-batch [doc0, doc0 + ndocs) (workspace wp) until the sub-batch's index counter runs out.
-// wb: the warp's shared memory (IndexSmem layout), bar / phase: the warp's mbarrier for the bulk copies.
+// The warp indexes documents of the sub-batch [doc0, doc0 + ndocs) (workspace work) until the sub-batch's index counter runs out.
+// wb: the warp's shared memory (IndexSmem layout).
 template <int MAXD>
-__device__ __forceinline__ void index_docs(const ChatParams& P, uint32_t doc0, uint32_t ndocs, const WorkPtrs& wp, uint8_t* wb, const IdTables* s_ids, uint64_t* bar, uint32_t& phase, int lane) {
+__device__ __forceinline__ void index_docs(const ChatParams& P, uint32_t doc0, uint32_t ndocs, uint8_t* work, uint8_t* wb, const IdTables* s_ids, int lane) {
   using C = Cls<MAXD>;
-  uint8_t* s_in = wb;
-  uint32_t* s_tw = (uint32_t*)(wb + C::kIn);
+  const WorkPtrs wp = carve(work, ndocs, layout_of<MAXD>());   // carved here, so the paired kernel keeps one stage's pointers live at a time
+  uint32_t* s_tw = (uint32_t*)wb;
   uint16_t* s_bs = (uint16_t*)(s_tw + C::kTok);   // running backslash count in front of each token; later overlaid by the lookup list
-  uint32_t* s_nc = (uint32_t*)(wb + C::kIn + C::kTok * 6);
+  uint32_t* s_nc = (uint32_t*)(wb + C::kTok * 6);
 
   // work fetch, one document ahead: the atomic and the location loads of document k+1 complete under the scan of document k
   uint32_t li = 0;
@@ -67,19 +69,10 @@ __device__ __forceinline__ void index_docs(const ChatParams& P, uint32_t doc0, u
       AIGW_NEXT_DOC();
       continue;
     }
-    // ---- stage 1: one bulk asynchronous copy stages the body (no load / store issue slots)
-    // (a caller that broke the 16-byte alignment contract gets an ordinary cooperative copy instead of a fault)
-    if ((reinterpret_cast<uintptr_t>(g) & 15u) == 0) {
-      if (lane == 0) { const uint32_t nbytes = (len + 15u) & ~15u; mbar_expect_tx(bar, nbytes); bulk_g2s(s_in, g, nbytes, bar); }
-      mbar_wait(bar, phase); phase ^= 1u;
-    } else {
-      for (uint32_t i = lane; i < len; i += 32) s_in[i] = g[i];
-      __syncwarp();
-    }
-    // the next document starts its way from DRAM to L2 now (its location was loaded before this one's copy was issued)
+    // the next document starts its way from DRAM to L2 now (its location was loaded under the previous document's scan)
     if (lane == 0 && nlen && nlen <= (uint32_t)MAXD && (reinterpret_cast<uintptr_t>(ng) & 15u) == 0) bulk_prefetch_l2(ng, (nlen + 15u) & ~15u);
-    // ---- stages 2 + 2.5: structural index (chat_stage.cuh)
-    const uint32_t ntw = index_doc<MAXD>(s_in, len, lane, s_tw, s_bs, s_nc, s_ids);
+    // ---- stages 1 + 2 + 2.5: structural index of the body, read from global memory (chat_stage.cuh)
+    const uint32_t ntw = index_doc<MAXD, kBodyGlobal>(g, len, lane, s_tw, s_bs, s_nc, s_ids);
     if (ntw & 0x80000000u) { if (lane == 0) { wp.ntok[li] = ntw; atomicAdd(&wp.bins[0], 1u); } AIGW_NEXT_DOC(); continue; }
     const uint32_t ntok = ntw & 0x3fffffffu;
     // ---- write the token words out, coalesced; histogram of token counts for the shape sort
@@ -94,22 +87,24 @@ __device__ __forceinline__ void index_docs(const ChatParams& P, uint32_t doc0, u
 #undef AIGW_NEXT_DOC
 }
 
+// Registers are held to 64 (min_ctas CTAs of WARPS warps = 32 warps per SM), so that the register file is not what caps the
+// residency the shared-memory layouts allow.  The 2048 class's index CTAs are small enough for 9 per SM (36 warps, what its staged
+// layout had at 56 registers), so its index kernel is held to 56.
+template <int WARPS>
+__host__ __device__ constexpr int min_ctas() { return 32 / WARPS; }
+
 template <int MAXD, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) chat_index_kernel(const __grid_constant__ ChatParams P, uint32_t doc0, uint32_t ndocs, uint8_t* work) {
+__global__ void __launch_bounds__(WARPS * 32, MAXD <= 2048 ? 9 : min_ctas<WARPS>()) chat_index_kernel(const __grid_constant__ ChatParams P, uint32_t doc0, uint32_t ndocs, uint8_t* work) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // CTA-shared tables: key/value id hash tables
   IdTables* s_ids = (IdTables*)smem;
-  uint64_t* s_bar = (uint64_t*)(smem + sizeof(IdTables));
   {
     const uint32_t* src = (const uint32_t*)id_tables_of(P.schema);
     for (uint32_t i = threadIdx.x; i < sizeof(IdTables) / 4; i += blockDim.x) ((uint32_t*)s_ids)[i] = src[i];
   }
-  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
   __syncthreads();
-  constexpr int kHdr = (int)((sizeof(IdTables) + 8 * WARPS + 15) & ~(size_t)15);
-  uint32_t phase = 0;
-  index_docs<MAXD>(P, doc0, ndocs, carve(work, ndocs, layout_of<MAXD>()), smem + kHdr + (size_t)warp * IndexSmem<MAXD>::kWarpBytes, s_ids, &s_bar[warp], phase, lane);
+  index_docs<MAXD>(P, doc0, ndocs, work, smem + sizeof(IdTables) + (size_t)warp * IndexSmem<MAXD>::kWarpBytes, s_ids, lane);
 }
 
 // ---- Ks: counting sort by token count (documents with the same count almost always have the same shape).  Every block
@@ -242,19 +237,27 @@ __global__ void __launch_bounds__(WARPS * 32) chat_emit_kernel(const __grid_cons
   emit_docs<MAXD>(P, doc0, ndocs, carve(work, ndocs, layout_of<MAXD>()), smem + kHdr + (size_t)warp * EmitSmem<MAXD>::kWarpBytes, s_lits, &s_bar[warp], phase, lane);
 }
 
-// ---- K1 + K3 paired: the index of sub-batch k+1 and the emit of sub-batch k share the SMs in one launch.  Index is bound by issue
-// and shared-memory work and uses about a third of HBM bandwidth; emit is bound by HBM bandwidth.  There is no data dependency
-// between the two (separate workspace slots), so each CTA holds the header of both (id tables, literal table) and a per-warp
-// region that is the union of the two layouts (s_in at offset 0 in both).  Even warps start on the index list, odd warps on the
-// emit list; a warp that drains its list joins the other one, so both lists finish together.
-template <int MAXD>
-struct PairSmem { static constexpr int kWarpBytes = IndexSmem<MAXD>::kWarpBytes > EmitSmem<MAXD>::kWarpBytes ? IndexSmem<MAXD>::kWarpBytes : EmitSmem<MAXD>::kWarpBytes; };
-template <int WARPS>
-__host__ __device__ constexpr size_t pair_hdr_bytes() { return (sizeof(IdTables) + sizeof(LitTable::bytes) + 8 * WARPS + 15) & ~(size_t)15; }
+// ---- K1 + K3 paired: the index of sub-batch k+1 and the emit of sub-batch k share the SMs in one launch.  There is no data
+// dependency between the two (separate workspace slots), so each CTA holds the header of both (id tables, literal table).  Its
+// first EW warps are emit warps: each has an EmitSmem region (the staged body among it) and an mbarrier, starts on the emit list
+// and joins the index list when the emit list runs out.  The other IW warps are index warps with an IndexSmem region, which has no
+// room for a body: they index until the index list runs out and then exit.  An index warp's region is a third to a half of an emit
+// warp's, so an SM keeps more warps resident than with CTAs of union-sized regions.  With IW = 0 every warp has an emit region
+// (the union of the two layouts), even warps start on the index list and odd warps on the emit list, and a warp that drains its
+// list joins the other one: the layout for classes where the split gains no residency.
+template <int EW>
+__host__ __device__ constexpr size_t pair_hdr_bytes() { return (sizeof(IdTables) + sizeof(LitTable::bytes) + 8 * EW + 15) & ~(size_t)15; }
+template <int MAXD, int EW, int IW>
+__host__ __device__ constexpr size_t pair_smem_bytes() { return pair_hdr_bytes<EW>() + (size_t)EmitSmem<MAXD>::kWarpBytes * EW + (size_t)IndexSmem<MAXD>::kWarpBytes * IW; }
+// an emit warp indexes in its own region once the emit list runs out
+static_assert(EmitSmem<2048>::kWarpBytes >= IndexSmem<2048>::kWarpBytes && EmitSmem<5120>::kWarpBytes >= IndexSmem<5120>::kWarpBytes &&
+              EmitSmem<9216>::kWarpBytes >= IndexSmem<9216>::kWarpBytes && EmitSmem<17408>::kWarpBytes >= IndexSmem<17408>::kWarpBytes &&
+              EmitSmem<33792>::kWarpBytes >= IndexSmem<33792>::kWarpBytes && EmitSmem<65536>::kWarpBytes >= IndexSmem<65536>::kWarpBytes,
+              "an emit warp's region must hold the index layout");
 
-template <int MAXD, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) chat_pair_kernel(const __grid_constant__ ChatParams P, uint32_t doc0_idx, uint32_t n_idx, uint8_t* work_idx,
-                                                               uint32_t doc0_emit, uint32_t n_emit, uint8_t* work_emit) {
+template <int MAXD, int EW, int IW>
+__global__ void __launch_bounds__((EW + IW) * 32, min_ctas<EW + IW>()) chat_pair_kernel(const __grid_constant__ ChatParams P, uint32_t doc0_idx, uint32_t n_idx, uint8_t* work_idx,
+                                                                                        uint32_t doc0_emit, uint32_t n_emit, uint8_t* work_emit) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   IdTables* s_ids = (IdTables*)smem;
@@ -265,17 +268,26 @@ __global__ void __launch_bounds__(WARPS * 32) chat_pair_kernel(const __grid_cons
     for (uint32_t i = threadIdx.x; i < sizeof(IdTables) / 4; i += blockDim.x) ((uint32_t*)s_ids)[i] = src[i];
     for (uint32_t i = threadIdx.x; i < sizeof(c_lits.bytes) / 4; i += blockDim.x) ((uint32_t*)s_lits)[i] = ((const uint32_t*)c_lits.bytes)[i];
   }
-  if (threadIdx.x == 0) { for (int w = 0; w < WARPS; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
+  if (threadIdx.x == 0) { for (int w = 0; w < EW; w++) mbar_init(&s_bar[w], 1); mbar_fence_init(); }
   __syncthreads();
-  uint8_t* wb = smem + pair_hdr_bytes<WARPS>() + (size_t)warp * PairSmem<MAXD>::kWarpBytes;
-  const WorkPtrs wi = carve(work_idx, n_idx, layout_of<MAXD>()), we = carve(work_emit, n_emit, layout_of<MAXD>());
-  uint32_t phase = 0;
-  if ((warp & 1) == 0) {
-    index_docs<MAXD>(P, doc0_idx, n_idx, wi, wb, s_ids, &s_bar[warp], phase, lane);
-    emit_docs<MAXD>(P, doc0_emit, n_emit, we, wb, s_lits, &s_bar[warp], phase, lane);
+  uint8_t* regions = smem + pair_hdr_bytes<EW>();
+  if constexpr (IW == 0) {
+    uint8_t* wb = regions + (size_t)warp * EmitSmem<MAXD>::kWarpBytes;
+    uint32_t phase = 0;
+    if ((warp & 1) == 0) {
+      index_docs<MAXD>(P, doc0_idx, n_idx, work_idx, wb, s_ids, lane);
+      emit_docs<MAXD>(P, doc0_emit, n_emit, carve(work_emit, n_emit, layout_of<MAXD>()), wb, s_lits, &s_bar[warp], phase, lane);
+    } else {
+      emit_docs<MAXD>(P, doc0_emit, n_emit, carve(work_emit, n_emit, layout_of<MAXD>()), wb, s_lits, &s_bar[warp], phase, lane);
+      index_docs<MAXD>(P, doc0_idx, n_idx, work_idx, wb, s_ids, lane);
+    }
+  } else if (warp < EW) {
+    uint8_t* wb = regions + (size_t)warp * EmitSmem<MAXD>::kWarpBytes;
+    uint32_t phase = 0;
+    emit_docs<MAXD>(P, doc0_emit, n_emit, carve(work_emit, n_emit, layout_of<MAXD>()), wb, s_lits, &s_bar[warp], phase, lane);
+    index_docs<MAXD>(P, doc0_idx, n_idx, work_idx, wb, s_ids, lane);
   } else {
-    emit_docs<MAXD>(P, doc0_emit, n_emit, we, wb, s_lits, &s_bar[warp], phase, lane);
-    index_docs<MAXD>(P, doc0_idx, n_idx, wi, wb, s_ids, &s_bar[warp], phase, lane);
+    index_docs<MAXD>(P, doc0_idx, n_idx, work_idx, regions + (size_t)EW * EmitSmem<MAXD>::kWarpBytes + (size_t)(warp - EW) * IndexSmem<MAXD>::kWarpBytes, s_ids, lane);
   }
 }
 
@@ -301,29 +313,35 @@ static size_t pair_sub_docs() {
   return env > 0 ? (size_t)env : kPairSubDocs;
 }
 
-// Warps per CTA of the paired kernel, per class: as many resident warps per SM as the serial index and emit kernels have
-// (H100: 228 KB of shared memory per SM, 1 KB reserved per CTA; the CTA header is 8 448 bytes of tables + one mbarrier per warp):
-//   class   per-warp union   serial index / emit      paired
-//   2048     5 808 B          8 CTAs x 4 = 32 warps    4 CTAs x 8  = 32 warps    54 976 B per CTA
-//   5120    10 416 B          5 CTAs x 4 = 20          2 CTAs x 10 = 20         112 688 B
-//   9216    16 560 B          6 CTAs x 2 = 12          3 CTAs x 4  = 12          74 720 B
-//   17408   30 560 B          3 CTAs x 2 = 6           3 CTAs x 2  = 6           69 584 B
-// 0: the class keeps the serial schedule.  At 33792 and 65536 a CTA of the union layout holds a single warp and fewer CTAs fit
-// an SM than emit alone has (3 vs 4 and 1 vs 2), so pairing would cut emit's residency.
-constexpr int pair_warps(int maxd) { return maxd <= 2048 ? 8 : maxd <= 5120 ? 10 : maxd <= 9216 ? 4 : maxd <= 17408 ? 2 : 0; }
+// Emit and index warps per CTA of the paired kernel, per class (H100: 228 KB of shared memory per SM, 1 KB reserved per CTA; the CTA
+// header is 8 448 bytes of tables + one mbarrier per emit warp; see DESIGN.md §4.1 for the per-warp regions):
+//   class   emit + index warps / CTA   CTAs x warps / SM    shared memory / CTA
+//   2048     8 + 0                      4 x 8  = 32          54 976 B
+//   5120     6 + 10                     2 x 16 = 32         109 712 B
+//   9216     4 + 4                      2 x 8  = 16         102 560 B
+//   17408    2 + 3                      2 x 5  = 10         105 568 B
+// At 2048 the pair is held to 4 CTAs by its 64 registers, not by shared memory, so a split would gain no warps and only take the
+// emit list away from half of them: every warp keeps the union region.  Paired calls of 459 752 bodies timed against the union
+// layout (DESIGN.md §4.1): 9216 5.78-5.83 vs 6.44-6.47 ms, 17408 8.16-8.19 vs 10.74-10.75 ms.
+// 0: the class keeps the serial schedule.  At 33792 and 65536 an emit warp's region alone is 53 424 and 101 040 B, so a paired CTA
+// of one emit and one index warp keeps fewer emit warps on an SM than the serial emit kernel does (2 vs 4 and 1 vs 2).
+constexpr int pair_emit_warps(int maxd) { return maxd <= 2048 ? 8 : maxd <= 5120 ? 6 : maxd <= 9216 ? 4 : maxd <= 17408 ? 2 : 0; }
+constexpr int pair_index_warps(int maxd) { return maxd <= 2048 ? 0 : maxd <= 5120 ? 10 : maxd <= 9216 ? 4 : maxd <= 17408 ? 3 : 0; }
 static int class_of(uint32_t max_len) { return max_len <= 2048 ? 2048 : max_len <= 5120 ? 5120 : max_len <= 9216 ? 9216 : max_len <= 17408 ? 17408 : max_len <= 33792 ? 33792 : 65536; }
 // one slot of the paired schedule: `sub` documents' intermediates, 256-byte aligned
 static size_t pair_slot_bytes(int maxd, size_t sub) { return (chat_work_bytes((uint32_t)maxd, sub) + 255) & ~(size_t)255; }
 
-template <int MAXD, int WARPS>
+// WI / WE: warps per CTA of the serial index / emit kernel
+template <int MAXD, int WI, int WE>
 static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, cudaEvent_t* ev, int ev_cap,
                               int* launches) {
   using C = Cls<MAXD>;
-  constexpr int PW = pair_warps(MAXD) > 0 ? pair_warps(MAXD) : 1;   // PW is only used when pair_warps(MAXD) > 0
-  constexpr size_t hdr1 = (sizeof(IdTables) + 8 * WARPS + 15) & ~(size_t)15, hdr3 = (sizeof(LitTable::bytes) + 8 * WARPS + 15) & ~(size_t)15;
-  const size_t smem1 = hdr1 + (size_t)IndexSmem<MAXD>::kWarpBytes * WARPS;
-  const size_t smem3 = hdr3 + (size_t)EmitSmem<MAXD>::kWarpBytes * WARPS;
-  constexpr size_t smemp = pair_hdr_bytes<PW>() + (size_t)PairSmem<MAXD>::kWarpBytes * PW;
+  constexpr bool kPair = pair_emit_warps(MAXD) > 0;
+  constexpr int EW = kPair ? pair_emit_warps(MAXD) : 1, IW = kPair ? pair_index_warps(MAXD) : 1, PW = EW + IW;   // used when kPair
+  constexpr size_t hdr1 = sizeof(IdTables), hdr3 = (sizeof(LitTable::bytes) + 8 * WE + 15) & ~(size_t)15;
+  const size_t smem1 = hdr1 + (size_t)IndexSmem<MAXD>::kWarpBytes * WI;
+  const size_t smem3 = hdr3 + (size_t)EmitSmem<MAXD>::kWarpBytes * WE;
+  constexpr size_t smemp = pair_smem_bytes<MAXD, EW, IW>();
   static_assert(smemp <= 227 * 1024, "paired kernel's shared memory exceeds a CTA's limit");
   static ClsConfig cfgs[kMaxDevices];
   static std::mutex mu;
@@ -332,18 +350,18 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
   {
     std::lock_guard<std::mutex> lk(mu);
     if (!cc.ready) {
-      cudaError_t e = cudaFuncSetAttribute(chat_index_kernel<MAXD, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1);
+      cudaError_t e = cudaFuncSetAttribute(chat_index_kernel<MAXD, WI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1);
       if (e != cudaSuccess) return e;
-      e = cudaFuncSetAttribute(chat_emit_kernel<MAXD, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3);
+      e = cudaFuncSetAttribute(chat_emit_kernel<MAXD, WE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3);
       if (e != cudaSuccess) return e;
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bps1, chat_index_kernel<MAXD, WARPS>, WARPS * 32, smem1);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bps1, chat_index_kernel<MAXD, WI>, WI * 32, smem1);
       if (e != cudaSuccess) return e;
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bps3, chat_emit_kernel<MAXD, WARPS>, WARPS * 32, smem3);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bps3, chat_emit_kernel<MAXD, WE>, WE * 32, smem3);
       if (e != cudaSuccess) return e;
-      if constexpr (pair_warps(MAXD) > 0) {
-        e = cudaFuncSetAttribute(chat_pair_kernel<MAXD, PW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemp);
+      if constexpr (kPair) {
+        e = cudaFuncSetAttribute(chat_pair_kernel<MAXD, EW, IW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemp);
         if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bpsp, chat_pair_kernel<MAXD, PW>, PW * 32, smemp);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cc.bpsp, chat_pair_kernel<MAXD, EW, IW>, PW * 32, smemp);
         if (e != cudaSuccess) return e;
       }
       if (cc.bps1 < 1) cc.bps1 = 1;
@@ -357,7 +375,7 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
   // P is chat_pair_kernel: the index of the next sub-batch and the emit of this one share the SMs.  The walk runs alone (its
   // registers make the register file the binding resource when it shares an SM).  Stage timing (ev) keeps the serial schedule
   // below, whose four launches per sub-batch are what the stage split is read from.
-  if constexpr (pair_warps(MAXD) > 0) {
+  if constexpr (kPair) {
     const size_t slot = (work_cap / 2) & ~(size_t)255;
     size_t sub = slot > (size_t)kWorkHdr + 256 ? (slot - kWorkHdr - 256) / work_per_doc(layout_of<MAXD>()) : 0;
     if (sub > pair_sub_docs()) sub = pair_sub_docs();
@@ -370,7 +388,7 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
       auto grid = [&](long long units, int warps, int bps) { long long g = (long long)sm_count * bps, want = (units + warps - 1) / warps; return (unsigned)(want < g ? want : g); };
       cudaError_t e;
       if ((e = cudaMemsetAsync(wk_of(0), 0, kWorkHdr, st)) != cudaSuccess) return e;
-      chat_index_kernel<MAXD, WARPS><<<grid(nd_of(0), WARPS, cc.bps1), WARPS * 32, smem1, st>>>(P, first, nd_of(0), wk_of(0));
+      chat_index_kernel<MAXD, WI><<<grid(nd_of(0), WI, cc.bps1), WI * 32, smem1, st>>>(P, first, nd_of(0), wk_of(0));
       int nl = 1;
       for (uint32_t k = 0; k < nsb; k++) {
         const uint32_t nd = nd_of(k), doc0 = first + (uint32_t)(k * sub);
@@ -382,9 +400,9 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
           // slot (k+1) mod 2 was last used by sub-batch k-1, whose emit ran in the previous paired launch
           const uint32_t nn = nd_of(k + 1);
           if ((e = cudaMemsetAsync(wk_of(k + 1), 0, kWorkHdr, st)) != cudaSuccess) return e;
-          chat_pair_kernel<MAXD, PW><<<grid((long long)nn + nd, PW, cc.bpsp), PW * 32, smemp, st>>>(P, doc0 + nd, nn, wk_of(k + 1), doc0, nd, wk);
+          chat_pair_kernel<MAXD, EW, IW><<<grid((long long)nn + nd, PW, cc.bpsp), PW * 32, smemp, st>>>(P, doc0 + nd, nn, wk_of(k + 1), doc0, nd, wk);
         } else {
-          chat_emit_kernel<MAXD, WARPS><<<grid(nd, WARPS, cc.bps3), WARPS * 32, smem3, st>>>(P, doc0, nd, wk);
+          chat_emit_kernel<MAXD, WE><<<grid(nd, WE, cc.bps3), WE * 32, smem3, st>>>(P, doc0, nd, wk);
         }
         nl += 3;
       }
@@ -403,17 +421,16 @@ static cudaError_t launch_cls(const ChatParams& P, uint32_t first, int device, i
     const uint32_t nd = (uint32_t)(P.n - rel < sub ? P.n - rel : sub);
     const WorkPtrs wp = carve(work, nd, layout_of<MAXD>());
     if ((e = cudaMemsetAsync(work, 0, kWorkHdr, st)) != cudaSuccess) return e;
-    long long want = ((long long)nd + WARPS - 1) / WARPS;
-    long long g1 = (long long)sm_count * cc.bps1; if (want < g1) g1 = want;
-    long long g3 = (long long)sm_count * cc.bps3; if (want < g3) g3 = want;
+    long long g1 = (long long)sm_count * cc.bps1; if (((long long)nd + WI - 1) / WI < g1) g1 = ((long long)nd + WI - 1) / WI;
+    long long g3 = (long long)sm_count * cc.bps3; if (((long long)nd + WE - 1) / WE < g3) g3 = ((long long)nd + WE - 1) / WE;
     const bool timed = ev && 4 * sb + 3 < ev_cap;
     if (timed) cudaEventRecord(ev[4 * sb + 0], st);
-    chat_index_kernel<MAXD, WARPS><<<(unsigned)g1, WARPS * 32, smem1, st>>>(P, doc0, nd, work);
+    chat_index_kernel<MAXD, WI><<<(unsigned)g1, WI * 32, smem1, st>>>(P, doc0, nd, work);
     if (timed) cudaEventRecord(ev[4 * sb + 1], st);
     { const unsigned gs = (nd + 8191) / 8192; chat_sort_kernel<<<gs < 32 ? gs : 32, kBins, 0, st>>>(wp.ntok, wp.bins, wp.cursor, wp.perm, nd); }
     if ((e = launch_chat_walk(P, doc0, nd, work, layout_of<MAXD>(), st, sm_count)) != cudaSuccess) return e;
     if (timed) cudaEventRecord(ev[4 * sb + 2], st);
-    chat_emit_kernel<MAXD, WARPS><<<(unsigned)g3, WARPS * 32, smem3, st>>>(P, doc0, nd, work);
+    chat_emit_kernel<MAXD, WE><<<(unsigned)g3, WE * 32, smem3, st>>>(P, doc0, nd, work);
     if (timed) cudaEventRecord(ev[4 * sb + 3], st);
     nl += 4;
   }
@@ -432,18 +449,18 @@ size_t chat_work_bytes(uint32_t max_len, size_t ndocs) {
 // workspace that lets a call of n documents run its schedule: two slots of the paired schedule, or one sub-batch
 size_t chat_work_bytes_for(uint32_t max_len, size_t n) {
   const int maxd = class_of(max_len);
-  if (pair_warps(maxd) > 0 && n >= kPairMinSubBatches * pair_sub_docs()) return 2 * pair_slot_bytes(maxd, pair_sub_docs()) + 512;
+  if (pair_emit_warps(maxd) > 0 && n >= kPairMinSubBatches * pair_sub_docs()) return 2 * pair_slot_bytes(maxd, pair_sub_docs()) + 512;
   return chat_work_bytes(max_len, n < 262144 ? n : 262144) + 512;
 }
 
 cudaError_t launch_chat_translate(const ChatParams& P, uint32_t max_len, int device, int sm_count, cudaStream_t st, uint8_t* work, size_t work_cap, int* launches,
                                   cudaEvent_t* ev, int ev_cap, uint32_t first) {
-  if (max_len <= 2048) return launch_cls<2048, 4>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
-  if (max_len <= 5120) return launch_cls<5120, 4>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
-  if (max_len <= 9216) return launch_cls<9216, 2>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
-  if (max_len <= 17408) return launch_cls<17408, 2>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
-  if (max_len <= 33792) return launch_cls<33792, 1>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
-  return launch_cls<65536, 1>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 2048) return launch_cls<2048, 4, 4>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 5120) return launch_cls<5120, 4, 4>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 9216) return launch_cls<9216, 4, 2>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 17408) return launch_cls<17408, 2, 2>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  if (max_len <= 33792) return launch_cls<33792, 2, 1>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
+  return launch_cls<65536, 1, 1>(P, first, device, sm_count, st, work, work_cap, ev, ev_cap, launches);
 }
 
 }  // namespace aigw

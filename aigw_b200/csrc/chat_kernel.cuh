@@ -2,7 +2,8 @@
 //
 // One warp per request body ("document"), persistent CTAs pulling documents from a global
 // counter.  Per document:
-//   stage 1  load      16-byte coalesced global loads → per-warp shared-memory copy of the body
+//   stage 1  load      16-byte global loads of each lane's 32 bytes per round straight into registers
+//                      (the fused small-batch kernel: a per-warp shared-memory copy of the body)
 //   stage 2  index     lane-local byte classification (32 B per lane per round), escape/quote
 //                      carry resolution with ballots, in-string prefix-xor, structural token list
 //   stage 3  validate  JSON grammar over the token list, bracket matching (jump table)

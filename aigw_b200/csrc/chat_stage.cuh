@@ -6,6 +6,46 @@
 
 namespace aigw {
 
+// Where index_doc reads the request body.  The fused small-batch kernel stages it in shared memory (its bodies are in mapped host
+// memory: one PCIe round trip, then every re-read is on chip).  The throughput index kernel reads it from global memory: it streams
+// the body once and its scattered re-reads (token bytes, escapes, id lookups) hit L1 / L2, so no per-warp copy of the body holds
+// shared memory and caps the warps an SM keeps resident.
+enum BodyIn { kBodyShared, kBodyGlobal };
+
+template <int SRC>
+__device__ __forceinline__ uint32_t body_byte(const uint8_t* in, uint32_t p) {
+  if constexpr (SRC == kBodyGlobal) return __ldg(in + p);
+  else return in[p];
+}
+
+// The two 16-byte blocks a lane's 32 bytes [base, base + 32) of a round start in.  Global bodies are read from the 16-byte
+// aligned blocks at or below them (a body may break the 16-byte alignment contract), and only a block that holds at least one byte
+// of [in, in + len) is read: such a block never crosses a page, so nothing past the caller's allocation is touched.
+struct RoundLd { uint4 a, b; };
+__device__ __forceinline__ uint4 ldg_block_of(const uint8_t* in, uint32_t base, uint32_t len) {
+  const uint32_t o = (uint32_t)(uintptr_t)in & 15u;   // block at body byte base - o: holds a body byte iff base < len + o
+  return base < len + o ? __ldg((const uint4*)(in - o + base)) : make_uint4(0, 0, 0, 0);
+}
+__device__ __forceinline__ RoundLd ldg_round(const uint8_t* in, uint32_t base, uint32_t len) {
+  return RoundLd{ldg_block_of(in, base, len), ldg_block_of(in, base + 16u, len)};
+}
+// the eight words of body bytes [base, base + 32) from the round's blocks; a body off its 16-byte alignment (o != 0, the same for
+// every lane) also reads the third block and realigns
+__device__ __forceinline__ void round_words(const uint8_t* in, uint32_t base, uint32_t len, const RoundLd& r, uint32_t w[8]) {
+  const uint32_t o = (uint32_t)(uintptr_t)in & 15u;
+  w[0] = r.a.x; w[1] = r.a.y; w[2] = r.a.z; w[3] = r.a.w; w[4] = r.b.x; w[5] = r.b.y; w[6] = r.b.z; w[7] = r.b.w;
+  if (o) {
+    const uint4 c = ldg_block_of(in, base + 32u, len);
+    const uint32_t x[12] = {r.a.x, r.a.y, r.a.z, r.a.w, r.b.x, r.b.y, r.b.z, r.b.w, c.x, c.y, c.z, c.w};
+    const uint32_t sh = (o & 3u) * 8u, q = o >> 2;
+    uint32_t y[11];
+#pragma unroll
+    for (int i = 0; i < 11; i++) y[i] = __funnelshift_r(x[i], x[i + 1], sh);
+#pragma unroll
+    for (int i = 0; i < 8; i++) w[i] = q == 0 ? y[i] : q == 1 ? y[i + 1] : q == 2 ? y[i + 2] : y[i + 3];
+  }
+}
+
 // 16 bytes starting at an arbitrary shared-memory address (buffers carry ≥ 4 bytes of slack)
 __device__ __forceinline__ uint4 lds16_unaligned(const uint8_t* p) {
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
@@ -32,11 +72,21 @@ __device__ __forceinline__ uint32_t ctl_msb(uint32_t w, uint32_t z) { return ~((
 // msb mask → 4-bit mask (byte k → bit k): the four products land on bits 28..31 without carries
 __device__ __forceinline__ uint32_t nib_from_msb(uint32_t t) { return (t * 0x00204081u) >> 28; }
 
-// the four bytes s[p .. p+4) are hex digits; s is 4-byte aligned shared memory readable up to s[(p & ~3) + 8).  Two aligned word
-// reads and a per-byte range test ('0'..'9', or 'a'..'f' after folding case) instead of four dependent byte loads.
+// the four bytes s[p .. p+4) are hex digits.  Shared: s is 4-byte aligned and readable up to s[(p & ~3) + 8).  Global: s[p .. p+4)
+// lie in the body, and the word after s + p's word is read only when it holds one of them.  Two aligned word reads and a per-byte
+// range test ('0'..'9', or 'a'..'f' after folding case) instead of four dependent byte loads.
+template <int SRC>
 __device__ __forceinline__ bool hex4_at(const uint8_t* s, uint32_t p) {
-  const uint32_t* w = (const uint32_t*)(s + (p & ~3u));
-  const uint32_t x = __funnelshift_r(w[0], w[1], (p & 3u) * 8u);
+  uint32_t x;
+  if constexpr (SRC == kBodyGlobal) {
+    const uintptr_t a = (uintptr_t)(s + p);
+    const uint32_t* w = (const uint32_t*)(a & ~(uintptr_t)3);
+    const uint32_t sh = ((uint32_t)a & 3u) * 8u;
+    x = __funnelshift_r(__ldg(w), sh ? __ldg(w + 1) : 0u, sh);
+  } else {
+    const uint32_t* w = (const uint32_t*)(s + (p & ~3u));
+    x = __funnelshift_r(w[0], w[1], (p & 3u) * 8u);
+  }
   const uint32_t z = x & 0x7f7f7f7fu, l = z | 0x20202020u;
   const uint32_t dig = (z + 0x50505050u) & ~(z + 0x46464646u);   // bit 7 of each byte: 0x30 <= z <= 0x39
   const uint32_t let = (l + 0x1f1f1f1fu) & ~(l + 0x19191919u);   // 0x61 <= l <= 0x66
@@ -47,11 +97,11 @@ __device__ __forceinline__ bool hex4_at(const uint8_t* s, uint32_t p) {
 // the owning lane's mask is broadcast and lane i handles its bit i, so a 28-byte cluster of punctuation between two
 // messages costs one pass of ~12 instructions instead of a 28-trip single-lane loop.
 
-// ---- stages 2 + 2.5 of one document, by one warp: structural index of the body staged at s_in[0, len) into token words
-// s_tw[0, ntok) (position | byte | id / run length | escape flags).  Returns ntok (| bit 30: whitespace outside strings), or
-// 0x80000000 | aigw_reason.
+// ---- stages 2 + 2.5 of one document, by one warp: structural index of the body s_in[0, len) (SRC: staged in shared memory or
+// in global memory) into token words s_tw[0, ntok) (position | byte | id / run length | escape flags).  Returns ntok (| bit 30:
+// whitespace outside strings), or 0x80000000 | aigw_reason.
 // s_bs: kTok halfwords (running backslash counts, later the lookup list); s_nc: one word per 1 KB round.
-template <int MAXD>
+template <int MAXD, int SRC>
 __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len, int lane, uint32_t* s_tw, uint16_t* s_bs, uint32_t* s_nc, const IdTables* s_ids) {
   using C = Cls<MAXD>;
   const uint32_t lt = (1u << lane) - 1u;
@@ -61,13 +111,23 @@ __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len,
   uint32_t flags = 0;  // bit0 ctrl in string, bit1 bad escape, bit2 token overflow
   uint32_t any_nc = 0; // some round holds a valid escape the encoder re-spells (warp-uniform)
   uint32_t ws_any = 0; // whitespace outside strings (per lane; reduced at the end)
+  // global bodies: the loads of round r + 1 are in flight while round r is classified
+  RoundLd nxt;
+  if constexpr (SRC == kBodyGlobal) nxt = ldg_round(s_in, lane << 5, len);
   for (uint32_t r = 0; r < rounds; r++) {
     const uint32_t rbase = r << 10;
     const uint32_t base = rbase + (lane << 5);
-    // bytes at or beyond len (stale shared memory) are masked out of every class
+    // bytes at or beyond len (stale shared memory, or the rest of a global body's last block) are masked out of every class
     const uint32_t valid = base + 32u <= len ? 0xffffffffu : (base >= len ? 0u : ((1u << (len - base)) - 1u));
-    const uint4 a = *(const uint4*)(s_in + base), b = *(const uint4*)(s_in + base + 16);
-    const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint32_t w[8];
+    if constexpr (SRC == kBodyGlobal) {
+      const RoundLd cur = nxt;
+      if (r + 1u < rounds) nxt = ldg_round(s_in, base + 1024u, len);
+      round_words(s_in, base, len, cur, w);
+    } else {
+      const uint4 a = *(const uint4*)(s_in + base), b = *(const uint4*)(s_in + base + 16);
+      w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+    }
     // every class mask of the lane's 32 bytes at once (classify.cuh: 8 bit planes, then LOP3s)
     const ByteClasses bc = classify32(w);
     const uint32_t mq = bc.quote & valid, mb = bc.bslash & valid, mctl = bc.ctl & valid;
@@ -118,10 +178,10 @@ __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len,
        // checked here: the walk decodes only the strings it echoes or looks up, and a key it skips must still be valid JSON
       uint32_t e = esc & ps; bool nc = false;
       while (e) {
-        const int j = __ffs(e) - 1; e &= e - 1; const uint32_t p = base + j, c = s_in[p];
+        const int j = __ffs(e) - 1; e &= e - 1; const uint32_t p = base + j, c = body_byte<SRC>(s_in, p);
         if (!(c == '"' || c == '\\' || c == 'n' || c == 'r' || c == 't')) {
           if (c == '/' || c == 'b' || c == 'f') nc = true;
-          else if (c == 'u' && p + 4u < len && hex4_at(s_in, p + 1)) nc = true;
+          else if (c == 'u' && p + 4u < len && hex4_at<SRC>(s_in, p + 1)) nc = true;
           else flags |= 2u;
         }
       }
@@ -159,7 +219,7 @@ __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len,
           const uint32_t mbL = __shfl_sync(FULL, mb, L), bsL = __shfl_sync(FULL, bs_lane, L);
           if ((mk >> lane) & 1u) {
             const uint32_t pos = rbase + (L << 5) + lane;
-            uint32_t tword = pos | ((uint32_t)s_in[pos] << 16);
+            uint32_t tword = pos | (body_byte<SRC>(s_in, pos) << 16);
             if ((sc >> lane) & 1u) { const uint32_t run = __ffs(~(sc >> lane)) - 1u; if (lane + run < 32u) tword |= run << 24; }  // a run that reaches the block end is measured by the walker
             const uint32_t slot = wq + __popc(mk & lt);
             s_tw[slot] = tword;
@@ -170,7 +230,7 @@ __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len,
         uint32_t m = mtok, wpos = wpos0;
         while (m) {
           const int j = __ffs(m) - 1; m &= m - 1;
-          uint32_t tword = (base + j) | ((uint32_t)s_in[base + j] << 16);
+          uint32_t tword = (base + j) | (body_byte<SRC>(s_in, base + j) << 16);
           if ((msc >> j) & 1u) { const uint32_t run = __ffs(~(msc >> j)) - 1u; if (j + run < 32u) tword |= run << 24; }
           s_tw[wpos] = tword;
           s_bs[wpos] = (uint16_t)(bs_lane + __popc(mb & ((1u << j) - 1u)));
@@ -235,7 +295,7 @@ __device__ __forceinline__ uint32_t index_doc(const uint8_t* s_in, uint32_t len,
       const uint32_t w = s_tw[i];
       const uint32_t o = (w & 0xffffu) + 1u, n = (s_tw[i + 1] & 0xffffu) - o;
       const bool is_key = i + 2 < ntok && ((s_tw[i + 2] >> 16) & 0xffu) == ':';
-      s_tw[i] = w | (lookup_id(s_ids, s_in + o, n, is_key) << 24);
+      s_tw[i] = w | (lookup_id<SRC == kBodyGlobal>(s_ids, s_in + o, n, is_key) << 24);
     }
     __syncwarp();
   }

@@ -3336,7 +3336,7 @@ __global__ void __launch_bounds__(32) AIGW_CAT(chat_small_kernel_g, AIGW_WALK_GR
   const IdTables* ids = (P.schema & AIGW_SCHEMA_MESSAGES) ? &g_small_ids_msg : (P.schema & 48) == AIGW_SCHEMA_RESP_AWS_BEDROCK ? &g_small_ids_resp : &g_small_ids;
 #endif
   const long long t1 = clock64();
-  const uint32_t ntok = index_doc<MAXD>(s_in, len, lane, s_tw, s_bs, s_nc, ids);
+  const uint32_t ntok = index_doc<MAXD, kBodyShared>(s_in, len, lane, s_tw, s_bs, s_nc, ids);
   __syncwarp();
   const long long t2 = clock64();
   if (lane == 0) {
