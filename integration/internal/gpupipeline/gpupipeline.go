@@ -122,25 +122,7 @@ func (p *Pipeline) TranslateRerank(be Backend, cfg *C.aigw_backend_cfg, body, sc
 	if rc := C.aigw_rerank_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
 		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
 	}
-	res := *out.results
-	r := Result{Status: int(res.status), Reason: int(res.reason), Unchanged: res.body_kind == C.AIGW_BODY_UNCHANGED}
-	if res.status == C.AIGW_DECLINED {
-		return r, ErrDeclined
-	}
-	if res.status != C.AIGW_OK {
-		return r, nil
-	}
-	pl, bl := int(res.path_len), int(res.body_len)
-	if pl+bl > len(scratch) {
-		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
-	}
-	copy(scratch, unsafe.Slice((*byte)(unsafe.Pointer(out.out)), int(out.out_used))[int(res.out_off):int(res.out_off)+pl+bl])
-	r.Path = scratch[:pl]
-	if !r.Unchanged {
-		r.Body = scratch[pl : pl+bl]
-	}
-	r.Model = body[int(res.model_off) : int(res.model_off)+int(res.model_len)]
-	return r, nil
+	return largeResult(&out, body, scratch)
 }
 
 // EmbeddingsBatcherMax is the largest /v1/embeddings body the batcher's translate pass holds; larger ones go to
@@ -163,6 +145,38 @@ func (p *Pipeline) TranslateEmbeddings(be Backend, cfg *C.aigw_backend_cfg, body
 	if rc := C.aigw_embeddings_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
 		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
 	}
+	return largeResult(&out, body, scratch)
+}
+
+// ChatBatcherMax is the largest /v1/chat/completions body the batcher's translate pass holds; larger ones to an OpenAI or Azure
+// OpenAI backend go to aigw_chat_translate_large_host (TranslateChat).
+const ChatBatcherMax = 65536
+
+// TranslateChat is Translate for a /v1/chat/completions backend: a body of up to ChatBatcherMax bytes joins the backend's batch as
+// before, and a larger one to an OpenAI or Azure OpenAI backend (an agent transcript that resends its tools, tool calls and tool
+// results, up to 16 MiB - 1) is streamed through one CTA by aigw_chat_translate_large_host with the same semantics: ParseBody's
+// verdict, the forced include_usage and the model override.  A larger body to any other backend declines, as it does today.  cfg
+// is the configuration the backend was registered with.  The large call's record lives in the context's pinned arena, so it is
+// copied into scratch; a scratch smaller than the record declines.
+func (p *Pipeline) TranslateChat(be Backend, cfg *C.aigw_backend_cfg, body, scratch []byte) (Result, error) {
+	if len(body) <= ChatBatcherMax || (cfg.schema != C.AIGW_SCHEMA_OPENAI && cfg.schema != C.AIGW_SCHEMA_AZURE_OPENAI) {
+		return p.Translate(be, body, scratch)
+	}
+	off, ln := C.uint64_t(0), C.uint32_t(len(body))
+	var out C.aigw_batch_out
+	p.bulkMu.Lock()
+	defer p.bulkMu.Unlock()
+	if rc := C.aigw_chat_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	r, err := largeResult(&out, body, scratch)
+	r.Stream = (*out.results).flags&1 != 0
+	return r, err
+}
+
+// largeResult is the Result of the one request of a *_translate_large_host call, its record copied into scratch.  Called with
+// bulkMu held: out points into the bulk context's pinned arena.
+func largeResult(out *C.aigw_batch_out, body, scratch []byte) (Result, error) {
 	res := *out.results
 	r := Result{Status: int(res.status), Reason: int(res.reason), Unchanged: res.body_kind == C.AIGW_BODY_UNCHANGED}
 	if res.status == C.AIGW_DECLINED {
