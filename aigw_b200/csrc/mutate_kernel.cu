@@ -18,6 +18,19 @@ __device__ __forceinline__ uint32_t bits_range(uint32_t lo, uint32_t hi) {  // b
   return a & ~b;
 }
 
+// whether the copy pieces spell the staged input; called by the whole warp, out of line so the copy path's code stays as it was
+__device__ __noinline__ bool pieces_equal_input(const uint8_t* s_text, const uint8_t* s_in, const uint32_t* s_psrc, const uint32_t* s_plen,
+                                                uint32_t np, int lane) {
+  uint32_t diff = 0, o = 0;
+  for (uint32_t p = 0; p < np; p++) {
+    const uint32_t src = s_psrc[p], l = s_plen[p];
+    const uint8_t* sp = (src & kText) ? s_text + (src & ~kText) : s_in + src;
+    for (uint32_t i = lane; i < l; i += 32) diff |= sp[i] != s_in[o + i];
+    o += l;
+  }
+  return !__any_sync(FULLM, diff);
+}
+
 template <int MAXD>
 struct Lay {
   static constexpr int kIn = ((MAXD + 1023) / 1024) * 1024 + 16;
@@ -234,6 +247,9 @@ __global__ void __launch_bounds__(WARPS * 32) body_mutate_kernel(const __grid_co
       }
     }
     np = __shfl_sync(FULLM, np, 0); total = __shfl_sync(FULLM, total, 0); perr = __shfl_sync(FULLM, perr, 0); changed = __shfl_sync(FULLM, changed, 0);
+    // flags bit0: the record is the input byte for byte.  Edits can rebuild it (a set to the value already there, a delete
+    // whose re-append lands on the same bytes), so a record of the input's length is compared with the staged input below.
+    const uint32_t same_rule = !changed ? 1u : total == len ? 2u : 0u;   // 1 identical, 2 compare, 0 different
     if (perr) { res.reason = AIGW_R_OPS; if (lane == 0) P.results[doc] = res; continue; }
     const uint32_t rec = (total + 15u) & ~15u;
     unsigned long long obase = 0;
@@ -262,7 +278,8 @@ __global__ void __launch_bounds__(WARPS * 32) body_mutate_kernel(const __grid_co
         o += l;
       }
     }
-    res.out_off = obase + P.out_bias; res.out_len = total; res.status = AIGW_OK; res.flags = changed ? 0 : 1;
+    const bool same = same_rule == 1u || (same_rule == 2u && pieces_equal_input(s_text, s_in, s_psrc, s_plen, np, lane));
+    res.out_off = obase + P.out_bias; res.out_len = total; res.status = AIGW_OK; res.flags = same ? 1 : 0;
     if (lane == 0) P.results[doc] = res;
     __syncwarp();
   }

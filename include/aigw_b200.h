@@ -357,7 +357,16 @@ int aigw_chat_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, c
  * Stream s consists of chunks [chunk_first[s], chunk_first[s+1]); chunk c is bytes
  * [chunk_off[c], chunk_off[c+1]) of `bytes`.  For every stream the kernel replays the reference's
  * per-chunk ResponseBody calls (carry of the partial last line included) and returns the
- * Override-accumulated usage plus the last seen response model span (offset into `bytes`).  */
+ * Override-accumulated usage plus the last seen response model span (offset into `bytes`).
+ * One warp scans a stream in tiles of 8192 bytes; each tile starts with the unterminated line the previous tile left.
+ * status AIGW_DECLINED (run the stock path for that stream) when:
+ *   - a line is longer than 8192 bytes with its '\n', or the unterminated tail is 8192 bytes or longer (the reference never
+ *     parses that tail, so this one decline is the kernel's alone);
+ *   - a tile holds more than 512 '\n' (only streams whose lines average under 16 bytes can reach this);
+ *   - a data line the kernel decodes has an escaped key, a duplicate known key, nesting too deep, an exponent or too many digits
+ *     in a float field, or a model string with a backslash.  Lines holding `"usage"` or `\u` and the last two data lines of a
+ *     tile are always decoded; the other lines of a tile only when neither of those two yields a model, or when the tile has
+ *     more than 64 `"usage"` / `\u` positions.  */
 typedef struct aigw_sse_result { aigw_usage usage; uint64_t model_off; uint32_t model_len; uint32_t status; } aigw_sse_result; /* 48 bytes */
 int aigw_sse_usage_device(aigw_ctx* ctx, const uint8_t* d_bytes, const uint64_t* d_chunk_off, const uint32_t* d_chunk_first,
                           uint32_t n_streams, aigw_sse_result* d_results, void* stream, float* kernel_ms);
