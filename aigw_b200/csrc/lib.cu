@@ -26,6 +26,7 @@
 #include "rerank_large_kernel.cuh"
 #include "emb_large_kernel.cuh"
 #include "chat_large_kernel.cuh"
+#include "responses_large_kernel.cuh"
 
 #include <mutex>
 
@@ -109,6 +110,8 @@ struct aigw_ctx {
   Scratch<uint8_t> d_el_ws;
   // large chat passthroughs (aigw_chat_translate_large_device): one workspace slice per CTA (tokens, jump table, escape counts, arguments)
   Scratch<uint8_t> d_cl_ws;
+  // large /v1/responses requests (aigw_responses_translate_large_device): one workspace slice per CTA (tokens, jump table, escape counts)
+  Scratch<uint8_t> d_rl_ws;
   PinnedScratch<uint8_t> h_small;   // small-batch path: tables + bodies, read by the kernel in place
   // chat workspace (intermediates of one sub-batch) + per-stage timing events
   Scratch<uint8_t> d_work;
@@ -1044,6 +1047,73 @@ int aigw_chat_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, c
   if (S.rc) return S.rc;
   float ms = 0;
   if (int rc = aigw_chat_translate_large_device(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
+  S.back(ctx->h_res.p, d_res, n);
+  S.back((uint64_t*)ctx->h_used_arr.p, d_used, 1);
+  if (int rc = S.wait()) return rc;
+  const uint64_t used = ctx->h_used_arr[0] < cap ? ctx->h_used_arr[0] : cap;
+  if (used) { CK(cudaMemcpyAsync(ctx->h_out, d_out, used, cudaMemcpyDeviceToHost, S.st)); CK(cudaStreamSynchronize(S.st)); }
+  out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = S.h2d + 8; out->d2h_bytes = S.d2h + used;
+  out->gpu_launches = 1; out->kernel_ms = ms;
+  return 0;
+}
+
+// ------------------------------------------------------------------ /v1/responses requests of any size below 16 MiB
+int aigw_responses_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                          const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                          aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  if (!ctx) return -2;
+  if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
+  ENTER_ON(stream);
+  ChatParams C;
+  fill_params(C, cfg);   // the ":path" (path.Join("/", prefix, "responses")) and the override exactly as the translate pass gets them
+  ChatLargeParams P;
+  P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.results = d_results;
+  P.out = d_out; P.out_capacity = out_capacity; P.out_used = (unsigned long long*)d_out_used;
+  P.call_reason = cfg && cfg->schema == AIGW_SCHEMA_RESPONSES_OPENAI ? 0u : (uint32_t)AIGW_R_SCHEMA;
+  P.azure = 0; P.cost_configured = 0;   // one backend; ParseBody forces no include_usage here
+  P.force_mutation = C.force_mutation ? 1u : 0u;
+  P.override_len = C.override_len;
+  P.override_ok = 1;
+  for (uint32_t i = 0; i < C.override_len; i++) { const uint32_t c = (uint8_t)C.override_model[i]; if (c < 0x20 || c > 0x7f || c == '"' || c == '\\') P.override_ok = 0; }
+  chat_large_lits(P, C.openai_path, C.prefix_len, C.override_model, C.override_len, C.api_version, C.version_len);
+  const uint32_t ml = max_len && max_len < (1u << 24) ? max_len : (1u << 24) - 1u;
+  P.tok_cap = chat_large_tok_cap(ml);
+  P.slice = responses_large_slice_bytes(ml);
+  const int grid = responses_large_grid(ctx->sm_count, ml);
+  CK(ctx->d_rl_ws.ensure((size_t)grid * P.slice));
+  P.ws = ctx->d_rl_ws;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_responses_large(P, grid, st)); return 0; });
+}
+
+int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                        const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  memset(out, 0, sizeof *out);
+  if (!ctx) return -2;
+  if (n == 0) return 0;
+  ENTER();
+  ChatParams C;
+  fill_params(C, cfg);
+  // every record fits its slot: the path, the body, and the override with the ,"model":"" around it
+  uint32_t max_len = 0;
+  uint64_t cap = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (offsets[i] & 15u) { ctx->err = "aigw_responses_translate_large_host: request starts must be 16-byte aligned"; return -2; }
+    if (lens[i] > max_len) max_len = lens[i];
+    cap += ((uint64_t)C.prefix_len + lens[i] + C.override_len + 16u + 15u) & ~15ull;
+  }
+  HostStage S(ctx);
+  const uint8_t* d_bodies = S.span(bodies, offsets, lens, n);
+  const uint64_t* d_off = S.in(offsets, n);
+  const uint32_t* d_len = S.in(lens, n);
+  uint8_t* d_out = S.out<uint8_t>(cap);
+  aigw_doc_result* d_res = S.out<aigw_doc_result>(n);
+  uint64_t* d_used = S.out<uint64_t>(1);
+  S.step([&] { CK(cudaMemsetAsync(d_used, 0, 8, S.st)); return 0; });
+  S.step([&] { CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result))); CK(ctx->h_out.ensure(cap)); CK(ctx->h_used_arr.ensure(8)); return 0; });
+  if (S.rc) return S.rc;
+  float ms = 0;
+  if (int rc = aigw_responses_translate_large_device(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
   S.back(ctx->h_res.p, d_res, n);
   S.back((uint64_t*)ctx->h_used_arr.p, d_used, 1);
   if (int rc = S.wait()) return rc;

@@ -174,6 +174,33 @@ func (p *Pipeline) TranslateChat(be Backend, cfg *C.aigw_backend_cfg, body, scra
 	return r, err
 }
 
+// ResponsesBatcherMax is the largest /v1/responses body the batcher's translate pass holds; larger ones to an OpenAI backend go
+// to aigw_responses_translate_large_host (TranslateResponses).
+const ResponsesBatcherMax = 65536
+
+// TranslateResponses is Translate for a /v1/responses backend: a body of up to ResponsesBatcherMax bytes joins the backend's batch
+// as before, and a larger one to the OpenAI backend (an agent loop that resends its whole transcript, function calls, their
+// outputs and encrypted reasoning on every turn, up to 16 MiB - 1) is streamed through one CTA by
+// aigw_responses_translate_large_host with the same semantics: ParseBody's verdict and the model override.  A larger body to any
+// other backend declines, as it does today.  cfg is the configuration the backend was registered with.  The large call's record
+// lives in the context's pinned arena, so it is copied into scratch, which must hold len(body) + len(model override) + the path
+// + 16 bytes; a smaller scratch declines.
+func (p *Pipeline) TranslateResponses(be Backend, cfg *C.aigw_backend_cfg, body, scratch []byte) (Result, error) {
+	if len(body) <= ResponsesBatcherMax || cfg.schema != C.AIGW_SCHEMA_RESPONSES_OPENAI {
+		return p.Translate(be, body, scratch)
+	}
+	off, ln := C.uint64_t(0), C.uint32_t(len(body))
+	var out C.aigw_batch_out
+	p.bulkMu.Lock()
+	defer p.bulkMu.Unlock()
+	if rc := C.aigw_responses_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	r, err := largeResult(&out, body, scratch)
+	r.Stream = (*out.results).flags&1 != 0
+	return r, err
+}
+
 // largeResult is the Result of the one request of a *_translate_large_host call, its record copied into scratch.  Called with
 // bulkMu held: out points into the bulk context's pinned arena.
 func largeResult(out *C.aigw_batch_out, body, scratch []byte) (Result, error) {
