@@ -128,6 +128,8 @@ def load_library():
     L.aigw_chat_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
     L.aigw_responses_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
     L.aigw_responses_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
+    L.aigw_completions_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
+    L.aigw_completions_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
     L.aigw_sse_usage_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
     L.aigw_sse_usage_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64),
                                       C.POINTER(C.c_uint64), C.POINTER(C.c_float)]
@@ -333,6 +335,23 @@ class Context:
         ms = C.c_float(0)
         self._check(self.L.aigw_responses_translate_large_device(self.h, C.byref(cfg), d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used, None,
                                                                  C.byref(ms) if timed else None), "responses_translate_large_device")
+        return ms.value
+
+    # ---- /v1/completions requests of any size below 16 MiB (one CTA streams one request)
+    def completions_translate_large_host(self, cfg, arena, offs, lens):
+        """Same results as chat_translate_host under AIGW_SCHEMA_COMPLETIONS_OPENAI, for bodies of 1 byte to 16 MiB - 1."""
+        return self._translate_host(self.L.aigw_completions_translate_large_host, "completions_translate_large_host", cfg, arena, offs, lens)
+
+    def completions_translate_large(self, cfg, bodies):
+        """list of bytes → the same dicts as chat_translate"""
+        arena, offs, lens = pack_bodies(bodies)
+        res, out, _ = self.completions_translate_large_host(cfg, arena, offs, lens)
+        return self._records(bodies, res, out)
+
+    def completions_translate_large_device(self, cfg, d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used, timed=True):
+        ms = C.c_float(0)
+        self._check(self.L.aigw_completions_translate_large_device(self.h, C.byref(cfg), d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used, None,
+                                                                   C.byref(ms) if timed else None), "completions_translate_large_device")
         return ms.value
 
     @staticmethod

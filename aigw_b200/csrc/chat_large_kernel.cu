@@ -141,6 +141,7 @@ __device__ __forceinline__ uint32_t clen(const char* k) { uint32_t n = 0; while 
 // the two on the translate pass's corpora under every OpenAI / Azure configuration.
 struct ClWalk {
   using Scratch = ClArgs;
+  static constexpr bool kFlatArrays = false;
   LDoc d;
   LDoc a;          // the "arguments" text in hand
   ClArgs A;

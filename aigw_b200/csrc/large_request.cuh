@@ -1,6 +1,7 @@
-// The stages that chat_large_kernel (chat_large_kernel.cu) and responses_large_kernel (responses_large_kernel.cu) share: one CTA
-// of 256 threads streams one request, persistent CTAs pulling requests from a counter.  Each kernel supplies only its walk and
-// plan (thread 0); the scan, the depth pass, the grammar check and the emit are this file's.
+// The stages that chat_large_kernel (chat_large_kernel.cu), responses_large_kernel (responses_large_kernel.cu) and
+// completions_large_kernel (completions_large_kernel.cu) share: one CTA of 256 threads streams one request, persistent CTAs pulling
+// requests from a counter.  Each kernel supplies only its walk and plan (thread 0); the scan, the depth pass, the grammar check
+// and the emit are this file's, and so is the flat-array stage that only a walker with kFlatArrays compiles in.
 //   scan      the body streams through in 8 KB tiles (32 bytes per thread), as in emb_large_kernel: escapes by the odd-run rule with
 //             a carry across threads and tiles, escape validation, in-string parity, token compaction.  Every token also gets the
 //             number of escaped bytes, and of escapes the encoder re-spells (\/ \b \f \u), in front of it: a string holds a
@@ -8,6 +9,9 @@
 //             declines (AIGW_R_ESCAPE): the translate pass declines one only in the strings it echoes.
 //   depth     bracket depth after every token by a block-wide prefix sum (depth above 48 declines), the grammar of every scalar,
 //             escaped keys (declined: AIGW_R_ESCAPE)
+//   flat      (kFlatArrays walkers only) every thread: each '[' whose tokens up to its ']' alternate scalar, ',', scalar, ... gets
+//             its jump and a flag byte (CL_FLAT, and CL_ALL_INT64 when every element is null or an int64 literal), by two
+//             block-wide max-scans; the grammar check steps over such an array in one move
 //   grammar   thread 0 checks the token grammar and writes the jump table (every bracket to its partner)
 //   walk      thread 0: the kernel's walker (cl_request_loop's Walk) checks the members over the jump table in the translate
 //             pass's order, and the kernel's cl_plan lays out the record as at most 12 copy ops (body spans and literals)
@@ -69,6 +73,11 @@ __device__ __forceinline__ bool lone_surrogate(const uint8_t* body, uint32_t len
   return false;
 }
 
+// the flat-array stage's flag byte of a '[' token
+enum : uint8_t { CL_FLAT = 1, CL_ALL_INT64 = 2 };
+static constexpr uint32_t kClFlatPer = 8;                          // consecutive tokens per thread
+static constexpr uint32_t kClFlatTile = kClThreads * kClFlatPer;   // tokens per round of the stage
+
 // ---------------------------------------------------------------- token view with a jump table
 // tw: position (24) | type (8) as the scan writes it; cum: escaped bytes / re-spelled escapes in front of the token; jmp: the
 // partner of every bracket.  ty() answers as the translate pass's Doc does: '"' for both quotes, a scalar's first byte.
@@ -96,8 +105,12 @@ struct LDoc {
 };
 
 // validate_tokens (chat_walk_impl.cuh) over an LDoc: the grammar of the token list and its jump table.  0, AIGW_R_SYNTAX or
-// AIGW_R_DEPTH.  `scalars`: check each scalar's grammar here (the body's were checked by the depth pass).
-__device__ int cl_validate(LDoc& d, uint32_t* open_idx, bool scalars) {
+// AIGW_R_DEPTH.  `scalars`: check each scalar's grammar here (the body's were checked by the depth pass).  kSkipFlat: a '[' that
+// cl_flat_arrays flagged CL_FLAT in `flat` is a whole value, its jump already written (flags are read at '[' tokens only).  Such an
+// array holds scalars and commas in the only order the grammar takes, and the depth pass has declined nesting above 48, so the
+// step gives the answer the token-by-token check would.
+template <bool kSkipFlat = false>
+__device__ int cl_validate(LDoc& d, uint32_t* open_idx, bool scalars, const uint8_t* flat = nullptr) {
   uint64_t isobj = 0;
   uint32_t depth = 0, i = 0;
   int st = 0;   // 0 value expected, 1 key or '}', 2 key, 3 ':', 4 ',' or close, 5 value or ']', 6 done
@@ -114,6 +127,7 @@ __device__ int cl_validate(LDoc& d, uint32_t* open_idx, bool scalars) {
     }
     if (b == '{' || b == '[') {
       if (!(st == 0 || st == 5)) return AIGW_R_SYNTAX;
+      if constexpr (kSkipFlat) if (b == '[' && (flat[i] & CL_FLAT)) { i = d.jmp[i] + 1u; st = depth ? 4 : 6; continue; }
       if (depth >= kChatLargeMaxDepth) return AIGW_R_DEPTH;
       open_idx[depth] = i;
       if (b == '{') { isobj |= 1ull << depth; st = 1; } else { isobj &= ~(1ull << depth); st = 5; }
@@ -153,12 +167,138 @@ struct ClRec {
   __device__ void lit(uint32_t id) { push(OP_LIT, S.lit_off[id], S.lit_len[id]); }
 };
 
+// openai_request_result (chat_walk_impl.cuh) after the model span and the stream flag, for the passthroughs whose ParseBody returns
+// no mutated body (/v1/responses, /v1/completions): ":path", then the body, its original bytes, or the model override spliced in.
+// Edit B of chat_large_kernel's cl_plan without edit A.  Walk::Top has model_raw: the "model" value token, null included (the
+// splice point), kNone when absent.  0 or the reason.
+template <class Walk>
+__device__ __forceinline__ int cl_openai_plan(const ChatLargeParams& P, Walk& W, const typename Walk::Top& t, ClRec& R) {
+  const LDoc& d = W.d;
+  const uint32_t len = d.len;
+  R.lit(CL_OPENAI_PATH);
+  R.S.path_len = R.olen;
+  if (P.override_len == 0) {
+    if (P.force_mutation) { R.body(0, len); R.S.body_kind = AIGW_BODY_BYTES; } else R.S.body_kind = AIGW_BODY_UNCHANGED;
+    return 0;
+  }
+  if (!P.override_ok) return AIGW_R_UNSUPPORTED_FIELD;
+  R.S.body_kind = AIGW_BODY_BYTES;
+  if (t.model_raw != kNone) {   // replace the value
+    R.body(0, d.tok(t.model_raw));
+    R.lit(CL_QUOTE); R.lit(CL_OVERRIDE); R.lit(CL_QUOTE);
+    R.body(W.is_str(t.model_raw) ? d.tok(t.model_raw + 1) + 1u : d.scalar_end(t.model_raw), len);
+  } else {                      // append at the root: sjson rebuilds it, so the bytes outside its braces go
+    const uint32_t root_close = d.jmp[0];
+    R.body(d.tok(0), d.tok(root_close));
+    if (root_close != 1u) R.lit(CL_COMMA);
+    R.lit(CL_MODEL_MEMBER); R.lit(CL_QUOTE); R.lit(CL_OVERRIDE); R.lit(CL_QUOTE);
+    R.body(d.tok(root_close), d.tok(root_close) + 1u);
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------- flat arrays (every thread)
+// The scalar at body[o] is an integer literal within int64, cp_int64's rule: an optional '-', digits only, and at most
+// 9223372036854775807 (…808 with the sign).  The depth pass has checked the scalar's grammar, so the digits end the number unless a
+// fraction or an exponent follows them.
+__device__ __forceinline__ bool cl_int64_literal(const uint8_t* s, uint32_t len, uint32_t o) {
+  const uint32_t i = o + (s[o] == '-' ? 1u : 0u);
+  uint32_t e = i;
+  while (e < len && e - i < 20u && s[e] - '0' < 10u) e++;
+  if (e == i || e - i > 19u) return false;
+  if (e < len && (s[e] == '.' || (s[e] | 0x20u) == 'e')) return false;
+  if (e - i < 19u) return true;
+  const char* lim = "9223372036854775808";   // -2^63; the positive bound is one less
+  int c = 0;
+  for (uint32_t q = 0; q < 19u && !c; q++) c = (int)s[i + q] - (int)lim[q];
+  return c < 0 || (c == 0 && i != o);
+}
+
+// Finds every flat array: a '[' at token a whose tokens up to its ']' at b alternate scalar, ',', scalar, ..., scalar (or none:
+// "[]").  A token is a stop when it is neither a scalar nor a comma, or breaks the alternation with its predecessor (scalar
+// scalar, ',' ',', '[' ','); a ']' whose predecessor is ',' is not flat.  An exclusive max-scan over the CTA, carried across
+// rounds of kClFlatTile tokens, gives each ']' the last stop before it; when that stop is a '[', the array is flat: the ']' thread
+// writes jmp[a] = b and flag[a] = CL_FLAT, with CL_ALL_INT64 when a second max-scan (the last scalar that is neither null nor an
+// int64 literal) lies before a.  The stage only accepts: an array it does not flag is checked token by token as before.  It
+// writes the flag of every '[' of the request (0 in the round of the '[', then the ']' thread's flag after that round's barrier),
+// so no flag of an earlier request survives in the reused slice.  Called by every thread after the depth pass has passed.
+__device__ __forceinline__ void cl_flat_arrays(const uint32_t* tokw, uint32_t* jmp, uint8_t* flag, const uint8_t* body, uint32_t len,
+                                               uint32_t ntok) {
+  __shared__ uint32_t s_stop[2][8], s_bad[2][8];
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  // carried across rounds: 2 * (1 + the index of the last stop) + (that stop is a '['), and 1 + the index of the last element
+  // that is neither null nor an int64 literal; 0 for none
+  uint32_t c_stop = 0, c_bad = 0, it = 0;
+  for (uint32_t t0 = 0; t0 < ntok; t0 += kClFlatTile, it ^= 1u) {
+    const uint32_t j0 = t0 + tid * kClFlatPer;
+    uint32_t w[kClFlatPer];
+    if (j0 + kClFlatPer <= ntok) {   // 32-byte aligned: the slice is, and j0 is a multiple of 8
+      const uint4 a = *(const uint4*)(tokw + j0), b = *(const uint4*)(tokw + j0 + 4);
+      w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+    } else {
+#pragma unroll
+      for (uint32_t k = 0; k < kClFlatPer; k++) w[k] = j0 + k < ntok ? tokw[j0 + k] : 0u;
+    }
+    const uint32_t pt0 = j0 && j0 <= ntok ? tokw[j0 - 1] >> 24 : 0u;
+    uint32_t stopm = 0, badm = 0, lstop = 0, lbad = 0, pt = pt0;
+#pragma unroll
+    for (uint32_t k = 0; k < kClFlatPer; k++) {
+      const uint32_t j = j0 + k, t = w[k] >> 24;
+      if (j < ntok) {
+        const bool stop = (t != T_SCALAR && t != ',') || (t == T_SCALAR && pt == T_SCALAR) || (t == ',' && (pt == ',' || pt == '['));
+        if (stop) { stopm |= 1u << k; lstop = 2u * (j + 1u) + (t == '[' ? 1u : 0u); }
+        if (t == '[') flag[j] = 0;
+        if (t == T_SCALAR) {
+          const uint32_t o = w[k] & 0xffffffu;
+          if (body[o] != 'n' && !cl_int64_literal(body, len, o)) { badm |= 1u << k; lbad = j + 1u; }
+        }
+      }
+      pt = t;
+    }
+    // block-wide exclusive max-scans of (lstop, lbad) over the threads, carried in from the earlier rounds
+    uint32_t is = lstop, ib = lbad;
+#pragma unroll
+    for (int dd = 1; dd < 32; dd <<= 1) {
+      const uint32_t xs = __shfl_up_sync(FULL, is, dd), xb = __shfl_up_sync(FULL, ib, dd);
+      if ((int)lane >= dd) { is = max(is, xs); ib = max(ib, xb); }
+    }
+    if (lane == 31) { s_stop[it][warp] = is; s_bad[it][warp] = ib; }
+    const uint32_t us = __shfl_up_sync(FULL, is, 1), ub = __shfl_up_sync(FULL, ib, 1);
+    __syncthreads();
+    uint32_t rs = c_stop, rb = c_bad;
+#pragma unroll
+    for (uint32_t k = 0; k < 8; k++) {
+      const uint32_t vs = s_stop[it][k], vb = s_bad[it][k];
+      if (k < warp) { rs = max(rs, vs); rb = max(rb, vb); }
+      c_stop = max(c_stop, vs); c_bad = max(c_bad, vb);
+    }
+    if (lane) { rs = max(rs, us); rb = max(rb, ub); }
+    pt = pt0;
+#pragma unroll
+    for (uint32_t k = 0; k < kClFlatPer; k++) {
+      const uint32_t j = j0 + k, t = w[k] >> 24;
+      if (j < ntok) {
+        if (t == ']' && (rs & 1u) && pt != ',') {
+          const uint32_t a = (rs >> 1) - 1u;
+          jmp[a] = j;
+          flag[a] = CL_FLAT | (rb <= a ? CL_ALL_INT64 : 0);
+        }
+        if ((stopm >> k) & 1u) rs = 2u * (j + 1u) + (t == '[' ? 1u : 0u);
+        if ((badm >> k) & 1u) rb = j + 1u;
+      }
+      pt = t;
+    }
+  }
+}
+
 // The request loop of a large-request kernel, one CTA per request.  Walk is the kernel's walker (thread 0):
 //   Scratch, static Scratch scratch(uint2* rest)   its scratch, in the part of the CTA's slice past the escape counts
 //   LDoc d; Scratch A; uint32_t* stk;               the request's tokens, the scratch, kChatLargeMaxDepth words of shared memory
 //   int reason, pending; decline(r); bad()          the first decline; a pending 422 / 500 (declined as AIGW_R_CONTENT)
 //   Top, bool scan_top(Top&)                        the top-level members: t.model (a string, or kNone), t.stream (kNone: absent)
 //   void check(const Top&)                          every further check, in the translate pass's order
+//   static constexpr bool kFlatArrays               run cl_flat_arrays after the depth pass and let the grammar check step over
+//                                                   the arrays it flags; Scratch then has `uint8_t* flag`, one byte per token
 // and cl_plan(P, W, t, stream, R) plans the record (0 or the reason).  Only requests whose grammar check passed reach scan_top.
 template <class Walk>
 __device__ __forceinline__ void cl_request_loop(const ChatLargeParams& P, ClShared& S) {
@@ -326,6 +466,11 @@ __device__ __forceinline__ void cl_request_loop(const ChatLargeParams& P, ClShar
       if (carry != 0 && tid == 0) atomicMin(&S.fail, (uint32_t)AIGW_R_E400_SYNTAX);
     }
     __syncthreads();
+    // ================================================================ flat arrays (every thread; kFlatArrays walkers only)
+    if constexpr (Walk::kFlatArrays) {
+      if (S.fail == kNone) cl_flat_arrays(tokw, jmp, args.flag, body, len, ntok);
+      __syncthreads();
+    }
     // ================================================================ grammar, then the kernel's walk and plan (thread 0)
     if (tid == 0) {
       int f = S.fail == kNone ? 0 : (int)S.fail;
@@ -333,7 +478,11 @@ __device__ __forceinline__ void cl_request_loop(const ChatLargeParams& P, ClShar
       W.d = LDoc{body, len, tokw, cum, jmp, ntok};
       W.A = args; W.stk = S.stk;
       ClRec R(S);
-      if (!f) { const int vr = cl_validate(W.d, S.stk, false); if (vr) f = vr == AIGW_R_SYNTAX ? AIGW_R_E400_SYNTAX : vr; }
+      if (!f) {
+        int vr;
+        if constexpr (Walk::kFlatArrays) vr = cl_validate<true>(W.d, S.stk, false, args.flag); else vr = cl_validate(W.d, S.stk, false);
+        if (vr) f = vr == AIGW_R_SYNTAX ? AIGW_R_E400_SYNTAX : vr;
+      }
       if (!f) {
         typename Walk::Top t;
         if (W.scan_top(t)) {

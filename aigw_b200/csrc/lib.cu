@@ -27,6 +27,7 @@
 #include "emb_large_kernel.cuh"
 #include "chat_large_kernel.cuh"
 #include "responses_large_kernel.cuh"
+#include "completions_large_kernel.cuh"
 
 #include <mutex>
 
@@ -112,6 +113,8 @@ struct aigw_ctx {
   Scratch<uint8_t> d_cl_ws;
   // large /v1/responses requests (aigw_responses_translate_large_device): one workspace slice per CTA (tokens, jump table, escape counts)
   Scratch<uint8_t> d_rl_ws;
+  // large /v1/completions requests (aigw_completions_translate_large_device): tokens, jump table, escape counts, flat-array flags
+  Scratch<uint8_t> d_cpl_ws;
   PinnedScratch<uint8_t> h_small;   // small-batch path: tables + bodies, read by the kernel in place
   // chat workspace (intermediates of one sub-batch) + per-stage timing events
   Scratch<uint8_t> d_work;
@@ -1057,19 +1060,34 @@ int aigw_chat_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, c
   return 0;
 }
 
-// ------------------------------------------------------------------ /v1/responses requests of any size below 16 MiB
-int aigw_responses_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
-                                          const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
-                                          aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+// ------------------------------------------------------------------ /v1/responses and /v1/completions requests of any size below 16 MiB
+// The OpenAI passthroughs whose ParseBody returns no mutated body: one kernel per schema on ChatLargeParams, each with its own
+// slice size, grid and context workspace.
+struct OpenAILarge {
+  int32_t schema;
+  const char* host_name;   // for the alignment error
+  uint64_t (*slice_bytes)(uint32_t);
+  int (*grid)(int, uint32_t);
+  cudaError_t (*launch)(const ChatLargeParams&, int, cudaStream_t);
+  Scratch<uint8_t> aigw_ctx::*ws;
+};
+static const OpenAILarge kResponsesLarge = {AIGW_SCHEMA_RESPONSES_OPENAI, "aigw_responses_translate_large_host", responses_large_slice_bytes,
+                                            responses_large_grid, launch_responses_large, &aigw_ctx::d_rl_ws};
+static const OpenAILarge kCompletionsLarge = {AIGW_SCHEMA_COMPLETIONS_OPENAI, "aigw_completions_translate_large_host", completions_large_slice_bytes,
+                                              completions_large_grid, launch_completions_large, &aigw_ctx::d_cpl_ws};
+
+static int openai_large_device(const OpenAILarge& K, aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                               const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                               aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
   if (!ctx) return -2;
   if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
   ENTER_ON(stream);
   ChatParams C;
-  fill_params(C, cfg);   // the ":path" (path.Join("/", prefix, "responses")) and the override exactly as the translate pass gets them
+  fill_params(C, cfg);   // the ":path" (path.Join("/", prefix, "responses" / "completions")) and the override exactly as the translate pass gets them
   ChatLargeParams P;
   P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.results = d_results;
   P.out = d_out; P.out_capacity = out_capacity; P.out_used = (unsigned long long*)d_out_used;
-  P.call_reason = cfg && cfg->schema == AIGW_SCHEMA_RESPONSES_OPENAI ? 0u : (uint32_t)AIGW_R_SCHEMA;
+  P.call_reason = cfg && cfg->schema == K.schema ? 0u : (uint32_t)AIGW_R_SCHEMA;
   P.azure = 0; P.cost_configured = 0;   // one backend; ParseBody forces no include_usage here
   P.force_mutation = C.force_mutation ? 1u : 0u;
   P.override_len = C.override_len;
@@ -1078,16 +1096,17 @@ int aigw_responses_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg*
   chat_large_lits(P, C.openai_path, C.prefix_len, C.override_model, C.override_len, C.api_version, C.version_len);
   const uint32_t ml = max_len && max_len < (1u << 24) ? max_len : (1u << 24) - 1u;
   P.tok_cap = chat_large_tok_cap(ml);
-  P.slice = responses_large_slice_bytes(ml);
-  const int grid = responses_large_grid(ctx->sm_count, ml);
-  CK(ctx->d_rl_ws.ensure((size_t)grid * P.slice));
-  P.ws = ctx->d_rl_ws;
+  P.slice = K.slice_bytes(ml);
+  const int grid = K.grid(ctx->sm_count, ml);
+  Scratch<uint8_t>& ws = ctx->*K.ws;
+  CK(ws.ensure((size_t)grid * P.slice));
+  P.ws = ws;
   if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
-  return timed(ctx, st, kernel_ms, [&] { CK(launch_responses_large(P, grid, st)); return 0; });
+  return timed(ctx, st, kernel_ms, [&] { CK(K.launch(P, grid, st)); return 0; });
 }
 
-int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
-                                        const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+static int openai_large_host(const OpenAILarge& K, aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                             const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
   memset(out, 0, sizeof *out);
   if (!ctx) return -2;
   if (n == 0) return 0;
@@ -1098,7 +1117,7 @@ int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* c
   uint32_t max_len = 0;
   uint64_t cap = 0;
   for (uint32_t i = 0; i < n; i++) {
-    if (offsets[i] & 15u) { ctx->err = "aigw_responses_translate_large_host: request starts must be 16-byte aligned"; return -2; }
+    if (offsets[i] & 15u) { ctx->err = std::string(K.host_name) + ": request starts must be 16-byte aligned"; return -2; }
     if (lens[i] > max_len) max_len = lens[i];
     cap += ((uint64_t)C.prefix_len + lens[i] + C.override_len + 16u + 15u) & ~15ull;
   }
@@ -1113,7 +1132,7 @@ int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* c
   S.step([&] { CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result))); CK(ctx->h_out.ensure(cap)); CK(ctx->h_used_arr.ensure(8)); return 0; });
   if (S.rc) return S.rc;
   float ms = 0;
-  if (int rc = aigw_responses_translate_large_device(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
+  if (int rc = openai_large_device(K, ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
   S.back(ctx->h_res.p, d_res, n);
   S.back((uint64_t*)ctx->h_used_arr.p, d_used, 1);
   if (int rc = S.wait()) return rc;
@@ -1122,6 +1141,28 @@ int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* c
   out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = S.h2d + 8; out->d2h_bytes = S.d2h + used;
   out->gpu_launches = 1; out->kernel_ms = ms;
   return 0;
+}
+
+int aigw_responses_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                          const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                          aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  return openai_large_device(kResponsesLarge, ctx, cfg, d_bodies, d_offsets, d_lens, n, max_len, d_out, out_capacity, d_results, d_out_used, stream, kernel_ms);
+}
+
+int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                        const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  return openai_large_host(kResponsesLarge, ctx, cfg, bodies, offsets, lens, n, out);
+}
+
+int aigw_completions_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                            const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                            aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  return openai_large_device(kCompletionsLarge, ctx, cfg, d_bodies, d_offsets, d_lens, n, max_len, d_out, out_capacity, d_results, d_out_used, stream, kernel_ms);
+}
+
+int aigw_completions_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                          const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  return openai_large_host(kCompletionsLarge, ctx, cfg, bodies, offsets, lens, n, out);
 }
 
 int aigw_sse_usage_device(aigw_ctx* ctx, const uint8_t* d_bytes, const uint64_t* d_chunk_off, const uint32_t* d_chunk_first,

@@ -32,6 +32,7 @@ struct RlScratch {};
 // has to be made in both; test_responses_large_gpu.py compares the two on the translate pass's corpora.
 struct RqWalk {
   using Scratch = RlScratch;
+  static constexpr bool kFlatArrays = false;
   LDoc d;
   Scratch A;
   uint32_t* stk;
@@ -264,33 +265,8 @@ struct RqWalk {
   __device__ void check(const Top&) {}   // every check ran in scan_top
 };
 
-// openai_request_result after the model span and the stream flag: ":path", then the body, its original bytes, or the model
-// override spliced in.  Edit B of chat_large_kernel's cl_plan without edit A (ParseBody returns no mutated body here).  0 or the
-// reason.
-__device__ int cl_plan(const ChatLargeParams& P, RqWalk& W, const RqWalk::Top& t, bool, ClRec& R) {
-  const LDoc& d = W.d;
-  const uint32_t len = d.len;
-  R.lit(CL_OPENAI_PATH);
-  R.S.path_len = R.olen;
-  if (P.override_len == 0) {
-    if (P.force_mutation) { R.body(0, len); R.S.body_kind = AIGW_BODY_BYTES; } else R.S.body_kind = AIGW_BODY_UNCHANGED;
-    return 0;
-  }
-  if (!P.override_ok) return AIGW_R_UNSUPPORTED_FIELD;
-  R.S.body_kind = AIGW_BODY_BYTES;
-  if (t.model_raw != kNone) {   // replace the value
-    R.body(0, d.tok(t.model_raw));
-    R.lit(CL_QUOTE); R.lit(CL_OVERRIDE); R.lit(CL_QUOTE);
-    R.body(W.is_str(t.model_raw) ? d.tok(t.model_raw + 1) + 1u : d.scalar_end(t.model_raw), len);
-  } else {                      // append at the root: sjson rebuilds it, so the bytes outside its braces go
-    const uint32_t root_close = d.jmp[0];
-    R.body(d.tok(0), d.tok(root_close));
-    if (root_close != 1u) R.lit(CL_COMMA);
-    R.lit(CL_MODEL_MEMBER); R.lit(CL_QUOTE); R.lit(CL_OVERRIDE); R.lit(CL_QUOTE);
-    R.body(d.tok(root_close), d.tok(root_close) + 1u);
-  }
-  return 0;
-}
+// openai_request_result after the model span and the stream flag (large_request.cuh)
+__device__ int cl_plan(const ChatLargeParams& P, RqWalk& W, const RqWalk::Top& t, bool, ClRec& R) { return cl_openai_plan(P, W, t, R); }
 
 __global__ void __launch_bounds__(kClThreads, 2) responses_large_kernel(const __grid_constant__ ChatLargeParams P) {
   __shared__ ClShared S;

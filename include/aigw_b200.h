@@ -114,7 +114,7 @@ enum aigw_schema { AIGW_SCHEMA_OPENAI = 0, AIGW_SCHEMA_AWS_BEDROCK = 1, AIGW_SCH
                     * []string / [][]int64 / []int64 (null elements allowed; a first element that is null, an object or a bool is a 400).
                     * DECLINED: a null root, "prompt":null, escaped keys and model, repeated known keys, float64 values (members, numbers
                     * in stop) with an exponent or more than 308 integer digits.  A token-id prompt costs two index tokens per id, so long ones decline with
-                    * AIGW_R_TOKENS (DESIGN.md §7). */
+                    * AIGW_R_TOKENS (DESIGN.md §7); aigw_completions_translate_large_* give their answers. */
                    AIGW_SCHEMA_COMPLETIONS = 256, AIGW_SCHEMA_COMPLETIONS_OPENAI = 256,
                    /* Cohere (filterapi.APISchemaCohere): a base schema of its own.  Alone it is no chat schema (DECLINED, AIGW_R_SCHEMA). */
                    AIGW_SCHEMA_COHERE = 7,
@@ -384,6 +384,39 @@ int aigw_responses_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg*
                                           aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
 int aigw_responses_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
                                         const uint32_t* lens, uint32_t n, aigw_batch_out* out);
+
+/* ---- /v1/completions requests of any size below 16 MiB to the OpenAI backend ----
+ * The translate pass declines every AIGW_SCHEMA_COMPLETIONS_OPENAI body above 64 KiB (AIGW_R_TOO_LARGE), and below it a token-id
+ * prompt beyond its index stage's token capacity (AIGW_R_TOKENS): fill-in-the-middle requests with a file or repository context in
+ * prompt and suffix, and prompts tokenized by the client ([]int64 or [][]int64; a 32 Ki-token context is about 190 KB).  These
+ * calls stream one request through one CTA and give the results of aigw_chat_translate_* for AIGW_SCHEMA_COMPLETIONS_OPENAI with
+ * the same configuration (status, reason class, ":path", body_kind, body bytes, model span, flags bit 0 stream, bit 1 never; 400s
+ * in the same body order), for bodies of 1 byte to 16 MiB - 1 (small ones included): ParseBody's verdict, then ":path" =
+ * path.Join("/", openai_prefix, "completions") and the body unchanged, its original bytes (force_body_mutation) or with the model
+ * override spliced (the first "model" value, or the member appended before the root's '}'); cost_configured is not read.  Flat
+ * arrays of numbers, null, true and false are checked by the whole CTA, so a token-id prompt costs about what a string prompt of
+ * its size does.  Arguments, records and results are those of aigw_chat_translate_device / _host; any other `cfg->schema`
+ * declines every body with AIGW_R_SCHEMA.  Where they differ from the translate pass (which may itself decline some of these for
+ * capacity):
+ *   AIGW_R_ESCAPE      also a key with a backslash anywhere (inside unknown members too), and a lone surrogate \u escape anywhere
+ *                      in the body
+ *   AIGW_R_TOO_LARGE   a body of 16 MiB or more, or a model above 65535 bytes
+ *   AIGW_R_TOKENS      more than len / 2 + 1024 scan tokens (structural bytes outside strings, both quotes of every string, the
+ *                      first byte of every scalar); a prompt of ids of three digits or more stays below it
+ *   AIGW_R_DEPTH       nesting deeper than 48 anywhere (the translate pass reports a syntax error that comes before it first)
+ *   AIGW_R_OUT_SPACE   (device form) the record does not fit out_capacity; body_len is set to the record length (path and body)
+ *                      it needs.  Records are bump-allocated in the order requests finish.  align16(path_len + len + override_len
+ *                      + 16) per body is always enough.
+ * Workspace slices are sized by the call's longest body (max_len; 0 = unknown: sized for 16 MiB): about 8.5 bytes per byte of it,
+ * within 1 GiB for the whole grid, and at most 2 CTAs per SM.  On 132 SMs a call whose longest body is up to about 470 KiB runs
+ * 264 CTAs; 1 MiB 120, 4 MiB 30, 8 MiB 15 and 16 MiB 7, whatever its other bodies are.  The host form is a staging wrapper around
+ * the device form: it sizes the output arena at align16(path_len + len + override_len + 16) per body, so it never declines for
+ * output space.  `out` stays valid until the next host-buffer call on the context.  Offsets must be multiples of 16. */
+int aigw_completions_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                            const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                            aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+int aigw_completions_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                          const uint32_t* lens, uint32_t n, aigw_batch_out* out);
 
 /* ---- OpenAI SSE response streams: usage scan (S1) + TokenUsage merge (C1) ----
  * Stream s consists of chunks [chunk_first[s], chunk_first[s+1]); chunk c is bytes

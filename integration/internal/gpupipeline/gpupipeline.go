@@ -201,6 +201,40 @@ func (p *Pipeline) TranslateResponses(be Backend, cfg *C.aigw_backend_cfg, body,
 	return r, err
 }
 
+// CompletionsBatcherMax is the largest /v1/completions body the batcher's translate pass holds; larger ones to an OpenAI backend
+// go to aigw_completions_translate_large_host (TranslateCompletions).
+const CompletionsBatcherMax = 65536
+
+// TranslateCompletions is Translate for a /v1/completions backend: a body of up to CompletionsBatcherMax bytes joins the backend's
+// batch as before, and a larger one to the OpenAI backend (a fill-in-the-middle request with a file or repository context, or a
+// prompt the client tokenized itself, up to 16 MiB - 1) is streamed through one CTA by aigw_completions_translate_large_host with
+// the same semantics: ParseBody's verdict and the model override.  A batched body that the translate pass declines with
+// AIGW_R_TOKENS (a token-id prompt beyond its index stage's token capacity) is retried there once.  A larger body to any other
+// backend declines, as it does today.  cfg is the configuration the backend was registered with.  The large call's record lives in
+// the context's pinned arena, so it is copied into scratch, which must hold len(body) + len(model override) + the path + 16 bytes;
+// a smaller scratch declines.
+func (p *Pipeline) TranslateCompletions(be Backend, cfg *C.aigw_backend_cfg, body, scratch []byte) (Result, error) {
+	if cfg.schema != C.AIGW_SCHEMA_COMPLETIONS_OPENAI {
+		return p.Translate(be, body, scratch)
+	}
+	if len(body) <= CompletionsBatcherMax {
+		r, err := p.Translate(be, body, scratch)
+		if r.Status != int(C.AIGW_DECLINED) || r.Reason != int(C.AIGW_R_TOKENS) {
+			return r, err
+		}
+	}
+	off, ln := C.uint64_t(0), C.uint32_t(len(body))
+	var out C.aigw_batch_out
+	p.bulkMu.Lock()
+	defer p.bulkMu.Unlock()
+	if rc := C.aigw_completions_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out); rc != 0 {
+		return Result{Status: int(C.AIGW_DECLINED)}, ErrDeclined
+	}
+	r, err := largeResult(&out, body, scratch)
+	r.Stream = (*out.results).flags&1 != 0
+	return r, err
+}
+
 // largeResult is the Result of the one request of a *_translate_large_host call, its record copied into scratch.  Called with
 // bulkMu held: out points into the bulk context's pinned arena.
 func largeResult(out *C.aigw_batch_out, body, scratch []byte) (Result, error) {
@@ -293,7 +327,9 @@ func ResponsesRequestSchema(backendSchema string) int {
 
 // CompletionsRequestSchema is the aigw_backend_cfg.schema of a /v1/completions request to a backend of that schema
 // (aigw_chat_translate_* or the batcher: CompletionsEndpointSpec.ParseBody + RequestBody, endpointspec.go:203-222), or -1 when the
-// backend has no translator for the endpoint (GetTranslator serves only OpenAI) and the stock path reports that error.
+// backend has no translator for the endpoint (GetTranslator serves only OpenAI) and the stock path reports that error.  Bodies above
+// 65 536 bytes, and token-id prompts beyond the translate pass's token capacity, go to aigw_completions_translate_large_host
+// through TranslateCompletions.
 func CompletionsRequestSchema(backendSchema string) int {
 	if backendSchema == "OpenAI" {
 		return C.AIGW_SCHEMA_COMPLETIONS_OPENAI
