@@ -864,8 +864,9 @@ struct Walker {
     if (msg >= 0 && d.str_len(msg) > 0) { pl.lit(L_ERR_MESSAGE); emit_str(msg); pl.lit(L_ERR_CLOSE); }
     else pl.lit(L_ERR_CLOSE_AFTER_CODE);
   }
-  // tokens_ok: the body is one well-formed JSON value
-  __device__ void plan_response_error(bool tokens_ok) {
+  // tokens_ok: the body is one well-formed JSON value; undecided: the reason the index or the grammar check gave up on a body that
+  // may still be JSON (0 when it did not)
+  __device__ void plan_response_error(bool tokens_ok, int undecided) {
     const int base = P->schema & 7;
     if (d.len == 0) { decline(AIGW_R_UNSUPPORTED_FIELD); return; }   // an empty error body is left to the stock path
     for (uint32_t i = 0; i < P->override_len; i++) { const uint32_t c = (uint8_t)P->override_model[i]; if (c < 0x20 || c > 0x7e || c == '"' || c == '\\') { decline(AIGW_R_UNSUPPORTED_FIELD); return; } }
@@ -882,6 +883,7 @@ struct Walker {
       return;
     }
     if (base == AIGW_SCHEMA_GCP_VERTEX) {
+      if (undecided) { decline(undecided); return; }   // a body that is not JSON becomes the message: that must be certain
       bool typed = tokens_ok; int msg = -1, status = -1;
       if (typed && !is_null(0)) {
         if (!is_obj(0)) typed = false;
@@ -3100,8 +3102,13 @@ static __device__ __forceinline__ void walk_doc(const ChatParams& P, const WalkB
     W.sc.p = B.scr; W.sc.n = 0; W.sc.cap = (uint32_t)B.kScr - 20u;
     W.tw_tail = B.tw + nt8; W.jmp_tail = B.jmp + nt8; W.tail_cap = B.kTok - (int)nt8;
     W.P = &P; W.reason = 0; W.pending = 0; W.stk = stk;
-    const bool tokens_ok = idx_ok && nt8 > 0 && validate_tokens(W.d, stk) == 0;
-    W.plan_response_error(tokens_ok);
+    const int vr = idx_ok && nt8 > 0 ? validate_tokens(W.d, stk) : 0;
+    const bool tokens_ok = idx_ok && nt8 > 0 && vr == 0;
+    // a raw control byte in a string, a body above the class, a token count above its capacity and nesting deeper than the walk's
+    // stack are no syntax errors (sonic decodes such a body), so the body is not known to be other than JSON
+    const uint32_t ir = nt_word & 0xffu;
+    const int undecided = !idx_ok && (ir == AIGW_R_CTRL_IN_STRING || ir == AIGW_R_TOO_LARGE || ir == AIGW_R_TOKENS) ? (int)ir : vr == AIGW_R_DEPTH ? vr : 0;
+    W.plan_response_error(tokens_ok, undecided);
     W.pl.flush();
     int reason = W.reason ? W.reason : W.pl.err;
     if (!reason && W.pl.nops == 0) reason = AIGW_R_OPS;

@@ -73,7 +73,7 @@ def chat_translate(schema, body: bytes, model_override="", prefix="v1", cost_con
     t = Translated()
     t.status, t.body_kind, t.stream = r.status, r.body_kind, bool(r.stream)
     t.body = C.string_at(r.body, r.body_len)
-    t.path = C.string_at(r.path, r.path_len).decode()
+    t.path = C.string_at(r.path, r.path_len).decode("utf-8", "surrogateescape")   # a model of invalid UTF-8 reaches the path as is
     t.model = C.string_at(r.model, r.model_len)
     t.err = C.string_at(r.err, r.err_len).decode("utf-8", "replace")
     t.mutated = C.string_at(r.mutated, r.mutated_len) if r.has_mutated else None
@@ -302,7 +302,7 @@ def messages_translate(schema, body: bytes, model_override="", api_version="", f
     t = Translated()
     t.status, t.body_kind, t.stream = r.status, r.body_kind, bool(r.stream)
     t.body = C.string_at(r.body, r.body_len)
-    t.path = C.string_at(r.path, r.path_len).decode()
+    t.path = C.string_at(r.path, r.path_len).decode("utf-8", "surrogateescape")   # a model of invalid UTF-8 reaches the path as is
     t.model = C.string_at(r.model, r.model_len)
     t.err = C.string_at(r.err, r.err_len).decode("utf-8", "replace")
     t.mutated = None
@@ -316,7 +316,7 @@ def embeddings_translate(schema, body: bytes, model_override="", prefix="v1", fo
     t = Translated()
     t.status, t.body_kind, t.stream = r.status, r.body_kind, False
     t.body = C.string_at(r.body, r.body_len)
-    t.path = C.string_at(r.path, r.path_len).decode()
+    t.path = C.string_at(r.path, r.path_len).decode("utf-8", "surrogateescape")   # a model of invalid UTF-8 reaches the path as is
     t.model = C.string_at(r.model, r.model_len)
     t.err = C.string_at(r.err, r.err_len).decode("utf-8", "replace")
     t.mutated = None

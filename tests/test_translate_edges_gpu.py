@@ -65,7 +65,11 @@ def to_dict(x, out, body):
 
 def run_paths(ctx, schema, bodies):
     """{path name: (class of each body in that path, results)}"""
-    cfg = cfg_of(ctx, schema)
+    return run_cfg_paths(ctx, cfg_of(ctx, schema), bodies)
+
+
+def run_cfg_paths(ctx, cfg, bodies):
+    """run_paths under a backend configuration of the caller's"""
     paths = {}
     try:
         ctx.chat_set_small_batch(0)
