@@ -37,6 +37,7 @@ struct ChatLargeParams {
   uint16_t lit_off[CL_COUNT];
   uint16_t lit_len[CL_COUNT];
   char lits[512];
+  uint32_t max_len;           // the call's longest request (chat_bedrock_large_kernel: the slice's layout)
 };
 
 static constexpr uint32_t kChatLargeMaxDepth = 48;

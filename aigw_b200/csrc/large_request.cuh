@@ -291,6 +291,12 @@ __device__ __forceinline__ void cl_flat_arrays(const uint32_t* tokw, uint32_t* j
   }
 }
 
+// A walker with `static constexpr bool kOwnRecord = true` takes over after the depth pass (and the flat-array stage):
+//   static void record(P, S, LDoc d, Scratch args, uint32_t doc)   called by every thread: the grammar check, its walk and plan,
+//                                                                  the request's result and its record
+template <class W, class = void> struct cl_own_record { static constexpr bool value = false; };
+template <class W> struct cl_own_record<W, decltype((void)W::kOwnRecord)> { static constexpr bool value = W::kOwnRecord; };
+
 // The request loop of a large-request kernel, one CTA per request.  Walk is the kernel's walker (thread 0):
 //   Scratch, static Scratch scratch(uint2* rest)   its scratch, in the part of the CTA's slice past the escape counts
 //   LDoc d; Scratch A; uint32_t* stk;               the request's tokens, the scratch, kChatLargeMaxDepth words of shared memory
@@ -471,79 +477,83 @@ __device__ __forceinline__ void cl_request_loop(const ChatLargeParams& P, ClShar
       if (S.fail == kNone) cl_flat_arrays(tokw, jmp, args.flag, body, len, ntok);
       __syncthreads();
     }
-    // ================================================================ grammar, then the kernel's walk and plan (thread 0)
-    if (tid == 0) {
-      int f = S.fail == kNone ? 0 : (int)S.fail;
-      Walk W;
-      W.d = LDoc{body, len, tokw, cum, jmp, ntok};
-      W.A = args; W.stk = S.stk;
-      ClRec R(S);
-      if (!f) {
-        int vr;
-        if constexpr (Walk::kFlatArrays) vr = cl_validate<true>(W.d, S.stk, false, args.flag); else vr = cl_validate(W.d, S.stk, false);
-        if (vr) f = vr == AIGW_R_SYNTAX ? AIGW_R_E400_SYNTAX : vr;
-      }
-      if (!f) {
-        typename Walk::Top t;
-        if (W.scan_top(t)) {
-          const bool stream = t.stream != kNone && W.d.ty(t.stream) == 't';
-          if (t.model != kNone) {
-            const uint32_t ml = W.d.str_len(t.model);
-            if (ml > 0xffffu) W.decline(AIGW_R_TOO_LARGE);   // model_len is 16 bits
-            else { S.model_off = W.d.str_off(t.model); S.model_len = ml; }
+    if constexpr (cl_own_record<Walk>::value) {
+      Walk::record(P, S, LDoc{body, len, tokw, cum, jmp, ntok}, args, doc);   // grammar, walk, plan and emit of its own
+    } else {
+      // ================================================================ grammar, then the kernel's walk and plan (thread 0)
+      if (tid == 0) {
+        int f = S.fail == kNone ? 0 : (int)S.fail;
+        Walk W;
+        W.d = LDoc{body, len, tokw, cum, jmp, ntok};
+        W.A = args; W.stk = S.stk;
+        ClRec R(S);
+        if (!f) {
+          int vr;
+          if constexpr (Walk::kFlatArrays) vr = cl_validate<true>(W.d, S.stk, false, args.flag); else vr = cl_validate(W.d, S.stk, false);
+          if (vr) f = vr == AIGW_R_SYNTAX ? AIGW_R_E400_SYNTAX : vr;
+        }
+        if (!f) {
+          typename Walk::Top t;
+          if (W.scan_top(t)) {
+            const bool stream = t.stream != kNone && W.d.ty(t.stream) == 't';
+            if (t.model != kNone) {
+              const uint32_t ml = W.d.str_len(t.model);
+              if (ml > 0xffffu) W.decline(AIGW_R_TOO_LARGE);   // model_len is 16 bits
+              else { S.model_off = W.d.str_off(t.model); S.model_len = ml; }
+            }
+            S.flags = stream ? 1u : 0u;
+            if (!W.bad()) W.check(t);
+            if (!W.bad() && W.pending) W.decline(AIGW_R_CONTENT);   // a 422 / internal error of another translator: outside the fast path
+            if (!W.bad()) { if (const int r = cl_plan(P, W, t, stream, R)) W.decline(r); }
           }
-          S.flags = stream ? 1u : 0u;
-          if (!W.bad()) W.check(t);
-          if (!W.bad() && W.pending) W.decline(AIGW_R_CONTENT);   // a 422 / internal error of another translator: outside the fast path
-          if (!W.bad()) { if (const int r = cl_plan(P, W, t, stream, R)) W.decline(r); }
+          f = W.reason;
+          if (!f && (R.full || R.n == 0)) f = AIGW_R_OPS;
         }
-        f = W.reason;
-        if (!f && (R.full || R.n == 0)) f = AIGW_R_OPS;
+        S.total = R.olen;
+        S.fail = f ? (uint32_t)f : kNone;
+        aigw_doc_result res;
+        res.out_off = 0; res.body_len = 0; res.path_len = 0; res.status = AIGW_DECLINED; res.reason = 0; res.model_off = 0; res.model_len = 0;
+        res.body_kind = AIGW_BODY_UNCHANGED; res.flags = 0; res.in_len = len; res._pad = 0;
+        if (f) {
+          res.reason = (uint8_t)f; res.status = f >= 48 ? AIGW_INTERNAL : f >= 40 ? AIGW_INVALID_422 : f >= 32 ? AIGW_MALFORMED_400 : AIGW_DECLINED;
+        } else {
+          const unsigned long long size = ((unsigned long long)R.olen + 15u) & ~15ull;
+          const unsigned long long o = atomicAdd(P.out_used, size);
+          if (o + size > P.out_capacity) { res.reason = AIGW_R_OUT_SPACE; res.body_len = R.olen; }   // the record length this request needs
+          else {
+            S.off = o;
+            res.out_off = o; res.path_len = (uint16_t)S.path_len; res.body_len = R.olen - S.path_len; res.status = AIGW_OK;
+            res.model_off = S.model_off; res.model_len = (uint16_t)S.model_len; res.body_kind = (uint8_t)S.body_kind; res.flags = (uint8_t)S.flags;
+          }
+        }
+        P.results[doc] = res;
       }
-      S.total = R.olen;
-      S.fail = f ? (uint32_t)f : kNone;
-      aigw_doc_result res;
-      res.out_off = 0; res.body_len = 0; res.path_len = 0; res.status = AIGW_DECLINED; res.reason = 0; res.model_off = 0; res.model_len = 0;
-      res.body_kind = AIGW_BODY_UNCHANGED; res.flags = 0; res.in_len = len; res._pad = 0;
-      if (f) {
-        res.reason = (uint8_t)f; res.status = f >= 48 ? AIGW_INTERNAL : f >= 40 ? AIGW_INVALID_422 : f >= 32 ? AIGW_MALFORMED_400 : AIGW_DECLINED;
-      } else {
-        const unsigned long long size = ((unsigned long long)R.olen + 15u) & ~15ull;
-        const unsigned long long o = atomicAdd(P.out_used, size);
-        if (o + size > P.out_capacity) { res.reason = AIGW_R_OUT_SPACE; res.body_len = R.olen; }   // the record length this request needs
+      __syncthreads();
+      if (S.off == ~0ull) continue;
+      // ================================================================ emit: 16-byte chunks, every thread busy
+      const uint32_t total = S.total, nchunk = (total + 15u) >> 4;
+      uint4* dst = (uint4*)(P.out + S.off);
+      for (uint32_t ch = tid; ch < nchunk; ch += kClThreads) {
+        const uint32_t o0 = ch << 4;
+        uint32_t k = 0;
+        while (S.op_end[k] <= o0) k++;
+        const uint32_t start = k ? S.op_end[k - 1] : 0u;
+        uint4 v;
+        if (S.op_kind[k] == OP_BODY && o0 + 16u <= S.op_end[k]) v = load16_unaligned(body + S.op_src[k] + (o0 - start));
         else {
-          S.off = o;
-          res.out_off = o; res.path_len = (uint16_t)S.path_len; res.body_len = R.olen - S.path_len; res.status = AIGW_OK;
-          res.model_off = S.model_off; res.model_len = (uint16_t)S.model_len; res.body_kind = (uint8_t)S.body_kind; res.flags = (uint8_t)S.flags;
+          unsigned long long lo = 0, hi = 0;   // zero past the record's end
+          uint32_t kk = k, st = start;
+          for (uint32_t b = 0; b < 16u && o0 + b < total; b++) {
+            const uint32_t o = o0 + b;
+            while (o >= S.op_end[kk]) { st = S.op_end[kk]; kk++; }
+            const uint32_t src = S.op_src[kk] + (o - st);
+            const unsigned long long x = S.op_kind[kk] == OP_BODY ? body[src] : S.lits[src];
+            if (b < 8u) lo |= x << (8u * b); else hi |= x << (8u * (b - 8u));
+          }
+          v = make_uint4((uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32));
         }
+        dst[ch] = v;
       }
-      P.results[doc] = res;
-    }
-    __syncthreads();
-    if (S.off == ~0ull) continue;
-    // ================================================================ emit: 16-byte chunks, every thread busy
-    const uint32_t total = S.total, nchunk = (total + 15u) >> 4;
-    uint4* dst = (uint4*)(P.out + S.off);
-    for (uint32_t ch = tid; ch < nchunk; ch += kClThreads) {
-      const uint32_t o0 = ch << 4;
-      uint32_t k = 0;
-      while (S.op_end[k] <= o0) k++;
-      const uint32_t start = k ? S.op_end[k - 1] : 0u;
-      uint4 v;
-      if (S.op_kind[k] == OP_BODY && o0 + 16u <= S.op_end[k]) v = load16_unaligned(body + S.op_src[k] + (o0 - start));
-      else {
-        unsigned long long lo = 0, hi = 0;   // zero past the record's end
-        uint32_t kk = k, st = start;
-        for (uint32_t b = 0; b < 16u && o0 + b < total; b++) {
-          const uint32_t o = o0 + b;
-          while (o >= S.op_end[kk]) { st = S.op_end[kk]; kk++; }
-          const uint32_t src = S.op_src[kk] + (o - st);
-          const unsigned long long x = S.op_kind[kk] == OP_BODY ? body[src] : S.lits[src];
-          if (b < 8u) lo |= x << (8u * b); else hi |= x << (8u * (b - 8u));
-        }
-        v = make_uint4((uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32));
-      }
-      dst[ch] = v;
     }
   }
 }

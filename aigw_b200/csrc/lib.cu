@@ -26,6 +26,7 @@
 #include "rerank_large_kernel.cuh"
 #include "emb_large_kernel.cuh"
 #include "chat_large_kernel.cuh"
+#include "chat_bedrock_large_kernel.cuh"
 #include "responses_large_kernel.cuh"
 #include "completions_large_kernel.cuh"
 
@@ -111,6 +112,8 @@ struct aigw_ctx {
   Scratch<uint8_t> d_el_ws;
   // large chat passthroughs (aigw_chat_translate_large_device): one workspace slice per CTA (tokens, jump table, escape counts, arguments)
   Scratch<uint8_t> d_cl_ws;
+  // large chat requests to AWS Bedrock (aigw_chat_bedrock_translate_large_device): chat_large's slice, then ops and scratch
+  Scratch<uint8_t> d_bl_ws;
   // large /v1/responses requests (aigw_responses_translate_large_device): one workspace slice per CTA (tokens, jump table, escape counts)
   Scratch<uint8_t> d_rl_ws;
   // large /v1/completions requests (aigw_completions_translate_large_device): tokens, jump table, escape counts, flat-array flags
@@ -912,22 +915,27 @@ int aigw_embeddings_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg
   return timed(ctx, st, kernel_ms, [&] { CK(launch_emb_large(P, grid, st)); return 0; });
 }
 
-int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
-                                         const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+using LargeDevice = int (*)(aigw_ctx*, const aigw_backend_cfg*, const uint8_t*, const uint64_t*, const uint32_t*, uint32_t, uint32_t, uint8_t*,
+                            uint64_t, aigw_doc_result*, uint64_t*, void*, float*);
+
+// The host form of a large-request device call whose records may exceed the first arena: Σ align16(path + k · len + 1024), the path
+// bounded by the longest configuration path (or the model, at most the body).  A request whose record did not fit reports the
+// length it needs, and those requests run once more into an arena of that size.
+static int large_host_retry(LargeDevice dev, const char* name, uint32_t k, aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies,
+                            const uint64_t* offsets, const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
   memset(out, 0, sizeof *out);
   if (!ctx) return -2;
   if (n == 0) return 0;
   ENTER();
   ChatParams C;
   fill_params(C, cfg);
-  // output arena: Σ align16(path + 2 · len + 1024), the path bounded by the longest configuration path (or the model, at most the body)
   const uint64_t path_max = (uint64_t)C.prefix_len + C.override_len + C.version_len + 64u;
   uint32_t max_len = 0;
   uint64_t cap = 0;
   for (uint32_t i = 0; i < n; i++) {
-    if (offsets[i] & 15u) { ctx->err = "aigw_embeddings_translate_large_host: request starts must be 16-byte aligned"; return -2; }
+    if (offsets[i] & 15u) { ctx->err = std::string(name) + ": request starts must be 16-byte aligned"; return -2; }
     if (lens[i] > max_len) max_len = lens[i];
-    cap += (path_max + 2ull * lens[i] + 1024u + 15u) & ~15ull;
+    cap += (path_max + (uint64_t)k * lens[i] + 1024u + 15u) & ~15ull;
   }
   HostStage S(ctx);
   const uint8_t* d_bodies = S.span(bodies, offsets, lens, n);
@@ -940,7 +948,7 @@ int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* 
   S.step([&] { CK(ctx->h_res.ensure((size_t)n * sizeof(aigw_doc_result))); CK(ctx->h_used_arr.ensure(8)); return 0; });
   if (S.rc) return S.rc;
   float ms = 0;
-  if (int rc = aigw_embeddings_translate_large_device(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
+  if (int rc = dev(ctx, cfg, d_bodies, d_off, d_len, n, max_len, d_out, cap, d_res, d_used, S.st, &ms)) return rc;
   S.back(ctx->h_res.p, d_res, n);
   S.back((uint64_t*)ctx->h_used_arr.p, d_used, 1);
   if (int rc = S.wait()) return rc;
@@ -976,7 +984,7 @@ int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* 
     if (S2.rc) return S2.rc;
     uint32_t ml2 = 0; for (uint32_t k = 0; k < m; k++) if (len2[k] > ml2) ml2 = len2[k];
     float ms2 = 0;
-    if (int rc = aigw_embeddings_translate_large_device(ctx, cfg, d_bodies, d_off2, d_len2, m, ml2, d_out2, cap2, d_res2, d_used2, S2.st, &ms2)) return rc;
+    if (int rc = dev(ctx, cfg, d_bodies, d_off2, d_len2, m, ml2, d_out2, cap2, d_res2, d_used2, S2.st, &ms2)) return rc;
     std::vector<aigw_doc_result> res2(m);
     uint64_t used2 = 0;
     S2.back(res2.data(), d_res2, m);
@@ -991,6 +999,11 @@ int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* 
   out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = h2d; out->d2h_bytes = d2h;
   out->gpu_launches = launches; out->kernel_ms = ms;
   return 0;
+}
+
+int aigw_embeddings_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                         const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  return large_host_retry(aigw_embeddings_translate_large_device, "aigw_embeddings_translate_large_host", 2, ctx, cfg, bodies, offsets, lens, n, out);
 }
 
 // ------------------------------------------------------------------ /v1/chat/completions passthroughs of any size below 16 MiB
@@ -1058,6 +1071,38 @@ int aigw_chat_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, c
   out->results = ctx->h_res; out->out = ctx->h_out; out->out_used = used; out->h2d_bytes = S.h2d + 8; out->d2h_bytes = S.d2h + used;
   out->gpu_launches = 1; out->kernel_ms = ms;
   return 0;
+}
+
+// ------------------------------------------------------------------ /v1/chat/completions to AWS Bedrock Converse of any size below 16 MiB
+int aigw_chat_bedrock_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                             const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                             aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  if (!ctx) return -2;
+  if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
+  ENTER_ON(stream);
+  ChatParams C;
+  fill_params(C, cfg);   // the override exactly as the translate pass gets it
+  ChatLargeParams P;
+  P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.results = d_results;
+  P.out = d_out; P.out_capacity = out_capacity; P.out_used = (unsigned long long*)d_out_used;
+  P.call_reason = cfg && cfg->schema == AIGW_SCHEMA_AWS_BEDROCK ? 0u : (uint32_t)AIGW_R_SCHEMA;
+  P.azure = 0; P.cost_configured = 0; P.force_mutation = 0; P.override_ok = 1;   // the Converse body is always rebuilt
+  P.override_len = C.override_len;
+  chat_large_lits(P, C.openai_path, C.prefix_len, C.override_model, C.override_len, C.api_version, C.version_len);
+  const uint32_t ml = max_len && max_len < (1u << 24) ? max_len : (1u << 24) - 1u;
+  P.max_len = ml;
+  P.tok_cap = chat_large_tok_cap(ml);
+  P.slice = chat_bedrock_large_slice_bytes(ml);
+  const int grid = chat_bedrock_large_grid(ctx->sm_count, ml);
+  CK(ctx->d_bl_ws.ensure((size_t)grid * P.slice));
+  P.ws = ctx->d_bl_ws;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_chat_bedrock_large(P, grid, st)); return 0; });
+}
+
+int aigw_chat_bedrock_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                           const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  return large_host_retry(aigw_chat_bedrock_translate_large_device, "aigw_chat_bedrock_translate_large_host", 3, ctx, cfg, bodies, offsets, lens, n, out);
 }
 
 // ------------------------------------------------------------------ /v1/responses and /v1/completions requests of any size below 16 MiB

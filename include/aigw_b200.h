@@ -353,6 +353,40 @@ int aigw_chat_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg,
 int aigw_chat_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
                                    const uint32_t* lens, uint32_t n, aigw_batch_out* out);
 
+/* ---- /v1/chat/completions requests of any size below 16 MiB to AWS Bedrock Converse ----
+ * The translate pass declines every chat body above 64 KiB (AIGW_R_TOO_LARGE), and aigw_chat_translate_large_* serves only the
+ * passthroughs.  These calls stream one request through one CTA and give the results of aigw_chat_translate_* for
+ * AIGW_SCHEMA_AWS_BEDROCK with the same configuration (status, reason class, ":path" /model/{PathEscape(model or override)}/converse
+ * or /converse-stream, body_kind AIGW_BODY_BYTES, the Converse body, model span, flags bit 0 stream; 400s in the same order, and a
+ * translator 422 / 500 reported as the translate pass reports it), for bodies of 1 byte to 16 MiB - 1 (small ones included).
+ * Arguments, records and results are those of aigw_chat_translate_device / _host; any other `cfg->schema` declines every body with
+ * AIGW_R_SCHEMA.  Where they differ from the translate pass (which may itself decline some of these for capacity):
+ *   AIGW_R_ESCAPE      the cases of aigw_chat_translate_large_*, and a backslash in an assistant content part's "type" or in a
+ *                      string "tool_choice"
+ *   AIGW_R_TOO_LARGE   a body of 16 MiB or more, a model above 65535 bytes, or a ":path" above 65535 bytes after PathEscape
+ *   AIGW_R_TOKENS      more than len / 2 + 1024 scan tokens
+ *   AIGW_R_DEPTH       nesting deeper than 48 anywhere
+ *   AIGW_R_SCRATCH     a tool call "arguments" string above 64 KiB, more than 256 KiB of them in one request, or more than 2^18
+ *                      units of key-order work over tool parameters and arguments objects (as aigw_chat_translate_large_*)
+ *   AIGW_R_OPS         more than len / 2 + 4096 copy ops in the record.  A body span is merged with the one it touches, so
+ *                      realistic requests stay far below it; a string that alternates re-spelled escapes (\/ \b \f \u) with
+ *                      single plain bytes costs two ops per three bytes and passes it at about 25 KB ("\/a" repeated 8228 times)
+ *   AIGW_R_OUT_SPACE   (device form) the record does not fit out_capacity; body_len is set to the record length (path and body) it
+ *                      needs.  A record above 2^32 - 16 bytes declines with body_len 0.  The record is not bounded by a small
+ *                      multiple of len: re-spelled escapes grow up to 3x (a backslash-b becomes a six-byte u-escape), and short
+ *                      messages gain their Converse literals (the empty tool message {"role":"tool","content":""} 2.4x)
+ * Workspace slices are sized by the call's longest body (max_len; 0 = unknown: sized for 16 MiB): about 19 bytes per byte of it plus
+ * 1.4 MB, within 1 GiB for the whole grid, and at most 2 CTAs per SM.  On 132 SMs a call whose longest body is up to about 128 KB
+ * runs 264 CTAs; 1 MiB 50, 4 MiB 13 and 16 MiB 3.  The host form is a staging wrapper around the device form: it sizes the output
+ * arena at align16(path + 3 * len + 1024) per body and runs the requests whose record did not fit once more into an arena of the
+ * lengths they reported, so it never declines for output space.  `out` stays valid until the next host-buffer call on the context.
+ * Offsets must be multiples of 16. */
+int aigw_chat_bedrock_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                             const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                             aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+int aigw_chat_bedrock_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                           const uint32_t* lens, uint32_t n, aigw_batch_out* out);
+
 /* ---- /v1/responses requests of any size below 16 MiB to the OpenAI backend ----
  * The translate pass declines every AIGW_SCHEMA_RESPONSES_OPENAI body above 64 KiB (AIGW_R_TOO_LARGE); agent loops resend the
  * whole transcript on every turn (instructions, tools, function_call / function_call_output pairs, reasoning items with their
