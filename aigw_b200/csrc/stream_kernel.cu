@@ -192,6 +192,7 @@ __device__ int an_event_core(StreamSlot& S, const uint8_t* et, uint32_t etl, con
   const bool ok = walk(data, (int)dl, g_an_schema.nodes, g_an_schema.fields, g_an_schema.keys, A_ROOT, cp);
   if (!ok) {  // syntax error ⇒ "unmarshal …" error; a well-formed value of another shape ⇒ unpinned, stock path
     int e = skip_any(data, 0, (int)dl);
+    if (e == -2) return AIGW_DECLINED;   // nesting beyond skip_any's levels: the decoder may accept it
     if (e >= 0) { while (e < (int)dl && ws(data[e])) e++; }
     return (e < 0 || e != (int)dl) ? AIGW_INTERNAL : AIGW_DECLINED;
   }
@@ -508,6 +509,7 @@ __device__ void step_aws_anthropic(StreamSlot& S, const StreamStep& st, uint8_t*
     uint8_t* pl = b + pos + 12 + hlen; const int pn = (int)(total - hlen - 16u);
     pos += total;                                          // the frame is consumed whatever it holds
     int e = skip_any(pl, 0, pn);
+    if (e == -2) { status = AIGW_DECLINED; break; }         // nested beyond skip_any's levels: not known to fail
     if (e < 0 || skipws(pl, e, pn) != pn) continue;        // json.Unmarshal error: the frame is skipped
     const int r0 = skipws(pl, 0, pn);
     if (pl[r0] != '{') continue;                           // null decodes to the zero struct, other roots fail: nothing to forward either way
@@ -614,6 +616,7 @@ __device__ int gem_decode(const uint8_t* p, int n, GemResp& g, bool buffered) {
   memset(&g, 0, sizeof g);
   int i = skipws(p, 0, n);
   const int root_end = skip_any(p, i, n);
+  if (root_end == -2) return 2;
   if (root_end < 0) return 1;
   if (!buffered && skipws(p, root_end, n) != n) return 1;
   if (p[i] == 'n') return 0;
@@ -862,6 +865,7 @@ __device__ bool n_usage(const uint8_t* p, int vs, int ve, NUsage& u) {
 // one `data: ` payload: 0 handled or ignored, 1 outside the subset
 __device__ int native_event(StreamSlot& S, const uint8_t* p, int n) {
   int e = skip_any(p, 0, n);
+  if (e == -2) return 1;
   if (e < 0) return 0;
   e = skipws(p, e, n);
   if (e != n) return 0;                                   // not one JSON value: the line is skipped

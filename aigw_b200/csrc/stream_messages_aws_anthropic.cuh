@@ -37,6 +37,7 @@ __device__ int mc_strings(const uint8_t* p, int vs, int ve, const char* names, i
 // json.Unmarshal(J, &MessagesStreamChunk{}) + reflectStreamingEvent: 0 decoded (et/etl = the event type), 1 outside the subset, 2 dropped
 __device__ int mc_chunk(StreamSlot& S, const uint8_t* p, int n, const uint8_t*& et, uint32_t& etl) {
   int e = skip_any(p, 0, n);
+  if (e == -2) return 1;                                  // nested beyond skip_any's levels
   if (e < 0 || skipws(p, e, n) != n) return 2;            // not one JSON value: json.Unmarshal fails
   const int r0 = skipws(p, 0, n);
   if (p[r0] != '{') return 1;
@@ -112,6 +113,7 @@ __device__ void step_messages_aws_anthropic(StreamSlot& S, const StreamStep& st,
     uint8_t* pl = b + pos + 12 + hlen; const int pn = (int)(total - hlen - 16u);
     pos += total;                                          // the frame is consumed whatever it holds
     int e = skip_any(pl, 0, pn);
+    if (e == -2) { status = AIGW_DECLINED; break; }         // nested beyond skip_any's levels: not known to fail
     if (e < 0 || skipws(pl, e, pn) != pn) continue;        // json.Unmarshal error: the frame is skipped
     const int r0 = skipws(pl, 0, pn);
     if (pl[r0] != '{') continue;

@@ -84,6 +84,9 @@ __device__ int o2a_block(StreamSlot& S, const uint8_t* blk, uint32_t bn, Wr& w) 
   const bool ok = walk(d, n, g_chunk_schema.nodes, g_chunk_schema.fields, g_chunk_schema.keys, N_ROOT, cp);
   if (cp.weird) return AIGW_DECLINED;
   if (!ok) return 0;                       // malformed chunks are skipped silently
+  // the walk bounds each skipped value to skip_any's 64 levels from its own start; jv_member / jv_next below skip whole members
+  // from the root, which can nest deeper than that: decline the chunk rather than read such a member as absent
+  if (skip_any(d, 0, n) == -2) return AIGW_DECLINED;
   const int r = jv_ws(d, 0, n);
   if (d[r] != '{') return 0;               // `null`: the zero chunk
   {
@@ -276,6 +279,7 @@ __device__ void step_messages_openai_buffered(StreamSlot& S, const StreamStep& s
   if (cp.weird) status = AIGW_DECLINED;
   else if (!ok) status = AIGW_INTERNAL;   // "failed to unmarshal OpenAI response"
   else if (cp.big) status = AIGW_DECLINED;
+  else if (skip_any(b, 0, n) == -2) status = AIGW_DECLINED;   // deeper than jv_member / jv_next can skip (see o2a_chunk)
   const uint8_t* mp = (const uint8_t*)S.model; uint32_t ml = S.model_len;
   if (!status) {
     const int r = jv_ws(b, 0, n);

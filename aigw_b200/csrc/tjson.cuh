@@ -36,7 +36,7 @@ struct CaptureT {
   uint32_t span_off[NSPANS], span_len[NSPANS];
   uint32_t span_set;       // bit i
   uint32_t span_esc;       // bit i: the captured string contains a backslash
-  uint32_t weird;          // escape in a key, duplicate known key, nesting too deep: caller must not trust the result
+  uint32_t weird;          // escape in a key, duplicate known key, nesting too deep (typed or skipped): caller must not trust the result
   uint32_t big;            // a captured integer does not fit in 31 bits
 };
 using Capture = CaptureT<2>;
@@ -127,7 +127,8 @@ __device__ inline bool f64_trunc_u32(const uint8_t* p, int i, int ie, int j, uin
   return true;
 }
 
-// Untyped value: syntax only.  Returns end index or -1.
+// Untyped value: syntax only.  Returns end index, -1 on a syntax error, or -2 when a container opens 65 deep inside the value (the
+// isobj bitmask holds 64 levels).  -2 is not a verdict on the text: the decoder accepts deeper nesting, so callers decline.
 __device__ inline int skip_any(const uint8_t* p, int i, int n) {
   uint64_t isobj = 0; int depth = 0;
   // state machine identical in spirit to validate_tokens, but byte driven
@@ -138,7 +139,7 @@ __device__ inline int skip_any(const uint8_t* p, int i, int n) {
     bool value_done = false;
     if (c == '"') { bool e = false; i = scan_string(p, i, n, e); if (i < 0) return -1; value_done = true; }
     else if (c == '{') {
-      if (depth >= 64) return -1;
+      if (depth >= 64) return -2;
       i++; while (i < n && ws(p[i])) i++;
       if (i < n && p[i] == '}') { i++; value_done = true; }
       else {
@@ -151,7 +152,7 @@ __device__ inline int skip_any(const uint8_t* p, int i, int n) {
         i++; continue;
       }
     } else if (c == '[') {
-      if (depth >= 64) return -1;
+      if (depth >= 64) return -2;
       i++; while (i < n && ws(p[i])) i++;
       if (i < n && p[i] == ']') { i++; value_done = true; }
       else { isobj &= ~(1ull << depth); depth++; continue; }
@@ -184,7 +185,8 @@ __device__ inline int skip_any(const uint8_t* p, int i, int n) {
 }
 
 // gjson.GetBytes(data, "type") on the object at p[i] == '{': the first top-level "type" member.  1: a string, its contents at
-// p[ts, ts+tl); 0: absent or not a string; -1: syntax error before it; -2: an escaped member name before it, or an escaped tag.
+// p[ts, ts+tl); 0: absent or not a string; -1: syntax error before it; -2: an escaped member name before it, an escaped tag, or a
+// member before it nested beyond skip_any's 64 levels.
 __device__ inline int union_tag(const uint8_t* p, int i, int n, int& ts, int& tl) {
   i++;
   for (;;) {
@@ -205,7 +207,7 @@ __device__ inline int union_tag(const uint8_t* p, int i, int n, int& ts, int& tl
       if (e2) return -2;
       ts = i + 1; tl = k - i - 2; return 1;
     }
-    i = skip_any(p, i, n); if (i < 0) return -1;
+    i = skip_any(p, i, n); if (i < 0) return i;
   }
 }
 
@@ -263,7 +265,9 @@ __device__ inline bool walk(const uint8_t* p, int n, const Node* nodes, const Fi
     }
     bool descend = false;
     if (nd.kind == K_ANY) {
-      const int j = skip_any(p, i, n); if (j < 0) return false;
+      const int j = skip_any(p, i, n);
+      if (j == -2) { cap.weird = 1; return false; }
+      if (j < 0) return false;
       if (nd.cap != 0xff) { const uint32_t s = nd.cap; cap.span_off[s] = i; cap.span_len[s] = j - i; cap.span_set |= 1u << s; }   // raw value (quotes included for strings)
       i = j;
     }

@@ -104,7 +104,7 @@ def _skip(p, i, depth=0):
         return _string(p, i)[0]
     if c in b"{[":
         if depth >= 64:
-            raise _Fail
+            raise _Out   # the library's untyped skip holds 64 levels; the decoder accepts deeper values
         close = 0x7D if c == 0x7B else 0x5D
         i = _ws(p, i + 1)
         if i < len(p) and p[i] == close:
