@@ -4,11 +4,12 @@
 //   ClWalkT<ClNoOut>   the dry plan: every check in the translate pass's order, nothing recorded.  chat_large_kernel runs it
 //                      before a passthrough, as the translate pass runs plan_bedrock with pl.dry.
 //   ClWalkT<ClOut>     the emitting plan: the same walk, and the Converse record as an unbounded list of copy ops in the CTA's
-//                      slice (chat_bedrock_large_kernel.cu).
+//                      slice (chat_large_record_impl.cuh, chat_bedrock_large_kernel.cu).  chat_anthropic_large_kernel.cu runs
+//                      the dry plan first and records the Anthropic Messages body with this walker's pieces.
 // A restatement of the translate pass, not a reuse: its Walker reads a 16-bit token word with key ids from its index stage and is
 // compiled once per schema group into its own kernels.  This one reads 24-bit positions and compares keys by their bytes.  A change
-// to ParseBody's checks or to plan_bedrock has to be made here too; test_chat_large_gpu.py and test_chat_bedrock_large_gpu.py
-// compare the two on the translate pass's corpora.
+// to ParseBody's checks or to plan_bedrock has to be made here too; test_chat_large_gpu.py, test_chat_bedrock_large_gpu.py and
+// test_chat_anthropic_large_gpu.py compare the two on the translate pass's corpora.
 #pragma once
 #include "canon_number.cuh"
 #include "chat_kernel.cuh"
@@ -153,6 +154,12 @@ enum ClTop : int {
 };
 
 __device__ __forceinline__ uint32_t clen(const char* k) { uint32_t n = 0; while (k[n]) n++; return n; }
+
+// the top-level members scan_top keeps (value tokens, kNone when absent or null); one type for every instantiation of the walk, so
+// that a dry walk and an emitting walk read the same scan
+struct ClTopMembers {
+  uint32_t model, messages, temperature, top_p, max_tokens, mct, stop, stream, stream_options, tools, tool_choice, thinking, service_tier, model_raw, so_raw;
+};
 
 // ---------------------------------------------------------------- the walk (thread 0)
 template <class Out>
@@ -459,7 +466,7 @@ struct ClWalkT {
     else decline(AIGW_R_E400_CONTENT);
   }
 
-  struct Top { uint32_t model, messages, temperature, top_p, max_tokens, mct, stop, stream, stream_options, tools, tool_choice, thinking, service_tier, model_raw, so_raw; };
+  using Top = ClTopMembers;
 
   __device__ int top_id(uint32_t m) const {
     const uint32_t n = d.str_len(m);

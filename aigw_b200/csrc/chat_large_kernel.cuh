@@ -37,7 +37,8 @@ struct ChatLargeParams {
   uint16_t lit_off[CL_COUNT];
   uint16_t lit_len[CL_COUNT];
   char lits[512];
-  uint32_t max_len;           // the call's longest request (chat_bedrock_large_kernel: the slice's layout)
+  uint32_t max_len;           // the call's longest request (the record kernels of chat_large_record.cuh: the slice's layout)
+  uint32_t gcp;               // chat_anthropic_large_kernel: AIGW_SCHEMA_GCP_ANTHROPIC, else AIGW_SCHEMA_AWS_ANTHROPIC
 };
 
 static constexpr uint32_t kChatLargeMaxDepth = 48;

@@ -387,6 +387,47 @@ int aigw_chat_bedrock_translate_large_device(aigw_ctx* ctx, const aigw_backend_c
 int aigw_chat_bedrock_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
                                            const uint32_t* lens, uint32_t n, aigw_batch_out* out);
 
+/* ---- /v1/chat/completions requests of any size below 16 MiB to Anthropic on GCP Vertex AI and AWS Bedrock ----
+ * The translate pass declines every chat body above 64 KiB (AIGW_R_TOO_LARGE); long-context prompts with cache_control on big
+ * system or user text blocks, and multi-turn transcripts with tool calls and tool results, are larger.  These calls stream one
+ * request through one CTA and give the results of aigw_chat_translate_* for AIGW_SCHEMA_GCP_ANTHROPIC / AIGW_SCHEMA_AWS_ANTHROPIC
+ * with the same configuration, for bodies of 1 byte to 16 MiB - 1 (small ones included): status and reason class (ParseBody's
+ * 400s in the same order, the "unsupported OpenAI content type" 500 and the invalid "arguments" 500, the temperature 422 after the
+ * message errors), the ":path" (GCP: publishers/anthropic/models/{model or override}:rawPredict or :streamRawPredict, raw; AWS:
+ * /model/{PathEscape(model or override)}/invoke or /invoke-with-response-stream), body_kind AIGW_BODY_BYTES, the Messages body
+ * (anthropic_version: cfg->api_version, or vertex-2023-10-16 / bedrock-2023-05-31), model span, flags bit 0 stream.  A non-empty
+ * "tools" declines at every size, as in the translate pass.  Arguments, records and results are those of aigw_chat_translate_device
+ * / _host; any other `cfg->schema` declines every body with AIGW_R_SCHEMA, and aigw_chat_translate_large_* and
+ * aigw_chat_bedrock_translate_large_* still decline these two schemas.  Where they differ from the translate pass (which may itself
+ * decline some of these for capacity):
+ *   AIGW_R_ESCAPE      the cases of aigw_chat_bedrock_translate_large_*, and a backslash in an assistant content part's "type"
+ *   AIGW_R_TOO_LARGE   a body of 16 MiB or more, a model above 65535 bytes, or a ":path" above 65535 bytes (GCP: raw, AWS: after
+ *                      PathEscape)
+ *   AIGW_R_TOKENS      more than len / 2 + 1024 scan tokens
+ *   AIGW_R_DEPTH       nesting deeper than 48 anywhere
+ *   AIGW_R_SCRATCH     a tool call "arguments" string above 64 KiB, more than 256 KiB of them in one request, more than 2^18 units of
+ *                      key-order work over arguments objects (as aigw_chat_bedrock_translate_large_*), or a string tool content whose
+ *                      first non-space byte is '{' or a backslash and whose unescaped text is above 64 KiB: its is_error flag needs
+ *                      it parsed, and this call parses it in the 64 KiB arguments buffer.  Such contents do not count against the
+ *                      256 KiB of arguments.
+ *   AIGW_R_OPS         more than len / 2 + 4096 copy ops in the record (as aigw_chat_bedrock_translate_large_*: "\/a" repeated in a
+ *                      user text passes it at about 25 KB)
+ *   AIGW_R_OUT_SPACE   (device form) the record does not fit out_capacity; body_len is set to the record length (path and body) it
+ *                      needs.  A record above 2^32 - 16 bytes declines with body_len 0.  The record is at most about 3.2 times len plus
+ *                      the path and a few hundred bytes: the densest is a run of the shortest tool messages ({"content":"x",
+ *                      "role":"tool"} becomes a 96-byte tool_result block); a backslash-b in a user text grows 3x.
+ * Workspace slices are those of aigw_chat_bedrock_translate_large_*: sized by the call's longest body (max_len; 0 = unknown: sized
+ * for 16 MiB), about 19 bytes per byte of it plus 1.4 MB, within 1 GiB for the whole grid, and at most 2 CTAs per SM.  On 132 SMs a
+ * call whose longest body is 128 KiB runs 264 CTAs; 1 MiB 50, 4 MiB 13 and 16 MiB 3.  The host form is a staging wrapper around the
+ * device form: it sizes the output arena at align16(path + 4 * len + 1024) per body and runs the requests whose record did not fit
+ * once more into an arena of the lengths they reported, so it never declines for output space.  `out` stays valid until the next
+ * host-buffer call on the context.  Offsets must be multiples of 16. */
+int aigw_chat_anthropic_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                               const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                               aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+int aigw_chat_anthropic_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                             const uint32_t* lens, uint32_t n, aigw_batch_out* out);
+
 /* ---- /v1/responses requests of any size below 16 MiB to the OpenAI backend ----
  * The translate pass declines every AIGW_SCHEMA_RESPONSES_OPENAI body above 64 KiB (AIGW_R_TOO_LARGE); agent loops resend the
  * whole transcript on every turn (instructions, tools, function_call / function_call_output pairs, reasoning items with their
