@@ -428,6 +428,48 @@ int aigw_chat_anthropic_translate_large_device(aigw_ctx* ctx, const aigw_backend
 int aigw_chat_anthropic_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
                                              const uint32_t* lens, uint32_t n, aigw_batch_out* out);
 
+/* ---- /v1/chat/completions requests of any size below 16 MiB to Gemini on GCP Vertex AI ----
+ * The translate pass declines every chat body above 64 KiB (AIGW_R_TOO_LARGE); Gemini's long context draws the largest ones: whole
+ * documents, long transcripts, many tool declarations.  These calls stream one request through one CTA and give the results of
+ * aigw_chat_translate_* for AIGW_SCHEMA_GCP_VERTEX with the same configuration, for bodies of 1 byte to 16 MiB - 1 (small ones
+ * included): status and reason class (ParseBody's 400s in the same order, the translator's 422 for a missing or null user / system
+ * content and for non-object "parameters" of a declaration without the JSON-schema form), the ":path"
+ * (publishers/google/models/{model or override}:generateContent or :streamGenerateContent?alt=sse, the model raw), body_kind
+ * AIGW_BODY_BYTES, the GenerateContent body ("contents" with consecutive user messages merged, "tools", "generation_config",
+ * "system_instruction"), model span, flags bit 0 stream.  As in the translate pass, tool messages, non-empty assistant "tool_calls",
+ * "tool_choice", "thinking", a non-empty "reasoning_effort", an empty or missing user text part, "parameters" outside the
+ * re-marshal subset (without the JSON-schema form), an integer field of more than 9 digits and a float field of more than 6
+ * significant digits (AIGW_R_NUMBER) decline.  Arguments, records and results are those of aigw_chat_translate_device / _host; any
+ * other `cfg->schema` declines every body with AIGW_R_SCHEMA, and the other large chat calls still decline AIGW_SCHEMA_GCP_VERTEX.
+ * Capacities: nesting depth 48, bodies of 16 MiB - 1, 64 members per object that is re-serialised with its keys sorted (tool
+ * parameters, and the arguments the dry Bedrock plan checks; AIGW_R_UNSUPPORTED_FIELD above, as in the translate pass), and the
+ * subset check's 24 pending schemas and 512 member visits per declaration (declined beyond, as in the translate pass).  Where they
+ * differ from the translate pass (which may itself decline some of these for capacity):
+ *   AIGW_R_ESCAPE      the cases of aigw_chat_bedrock_translate_large_*, and a backslash in an assistant content part's "type"
+ *   AIGW_R_TOO_LARGE   a body of 16 MiB or more, a model above 65535 bytes, or a ":path" above 65535 bytes (the model raw)
+ *   AIGW_R_TOKENS      more than len / 2 + 1024 scan tokens
+ *   AIGW_R_DEPTH       nesting deeper than 48 anywhere
+ *   AIGW_R_SCRATCH     a tool call "arguments" string above 64 KiB or more than 256 KiB of them in one request (the dry Bedrock plan
+ *                      parses them before the Gemini plan declines the tool call), or more than 2^18 units of key-order work
+ *                      (kChatAnyWork) over tool parameters and arguments objects, counted once for the dry plan and once for the
+ *                      Gemini plan
+ *   AIGW_R_OPS         more than len / 2 + 4096 copy ops in the record ("\/a" repeated in a user text passes it at about 25 KB)
+ *   AIGW_R_OUT_SPACE   (device form) the record does not fit out_capacity; body_len is set to the record length (path and body) it
+ *                      needs.  A record above 2^32 - 16 bytes declines with body_len 0.  The record is at most about 3.0 times len
+ *                      plus the path and a few hundred bytes: the densest is a user text of backslash-b escapes, each re-spelled as
+ *                      a six-byte u-escape; short messages shrink or keep their size ({"role":"user","content":"x"} becomes a
+ *                      merged {"text":"x"} part, {"role":"assistant"} becomes {"role":"model"}).
+ * Workspace slices are those of aigw_chat_bedrock_translate_large_* (about 19 bytes per byte of max_len plus 1.4 MB, within 1 GiB
+ * for the whole grid, at most 2 CTAs per SM), in the context's workspace of aigw_chat_anthropic_translate_large_*: the two calls
+ * share it.  The host form is a staging wrapper around the device form: it sizes the output arena at align16(path + 3 * len + 1024)
+ * per body and runs the requests whose record did not fit once more into an arena of the lengths they reported, so it never
+ * declines for output space.  `out` stays valid until the next host-buffer call on the context.  Offsets must be multiples of 16. */
+int aigw_chat_gemini_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                            const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                            aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms);
+int aigw_chat_gemini_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                          const uint32_t* lens, uint32_t n, aigw_batch_out* out);
+
 /* ---- /v1/responses requests of any size below 16 MiB to the OpenAI backend ----
  * The translate pass declines every AIGW_SCHEMA_RESPONSES_OPENAI body above 64 KiB (AIGW_R_TOO_LARGE); agent loops resend the
  * whole transcript on every turn (instructions, tools, function_call / function_call_output pairs, reasoning items with their

@@ -150,7 +150,8 @@ func (p *Pipeline) TranslateEmbeddings(be Backend, cfg *C.aigw_backend_cfg, body
 
 // ChatBatcherMax is the largest /v1/chat/completions body the batcher's translate pass holds; larger ones to an OpenAI or Azure
 // OpenAI backend go to aigw_chat_translate_large_host, to an AWS Bedrock backend to aigw_chat_bedrock_translate_large_host, to an
-// Anthropic backend on GCP Vertex AI or AWS Bedrock to aigw_chat_anthropic_translate_large_host (TranslateChat).
+// Anthropic backend on GCP Vertex AI or AWS Bedrock to aigw_chat_anthropic_translate_large_host, to a Gemini backend on GCP Vertex
+// AI to aigw_chat_gemini_translate_large_host (TranslateChat).
 const ChatBatcherMax = 65536
 
 // TranslateChat is Translate for a /v1/chat/completions backend: a body of up to ChatBatcherMax bytes joins the backend's batch as
@@ -159,15 +160,17 @@ const ChatBatcherMax = 65536
 // aigw_chat_translate_large_host (ParseBody's verdict, the forced include_usage and the model override), to an AWS Bedrock backend
 // by aigw_chat_bedrock_translate_large_host (ParseBody's verdict and the Converse request, its 422 / 500 answers included), to an
 // Anthropic backend on GCP Vertex AI or AWS Bedrock by aigw_chat_anthropic_translate_large_host (ParseBody's verdict and the
-// Messages request, its 422 / 500 answers included).  A larger body to any other backend (GCP Vertex AI Gemini) declines, as it
-// does today.  cfg is the configuration the backend was registered with.  The large call's record lives in the context's pinned
+// Messages request, its 422 / 500 answers included), to a Gemini backend on GCP Vertex AI by aigw_chat_gemini_translate_large_host
+// (ParseBody's verdict and the GenerateContent request, its 422 answers included).  No chat backend declines a body for its size
+// any more.  cfg is the configuration the backend was registered with.  The large call's record lives in the context's pinned
 // arena, so it is copied into scratch; a scratch smaller than the record declines.
 func (p *Pipeline) TranslateChat(be Backend, cfg *C.aigw_backend_cfg, body, scratch []byte) (Result, error) {
 	if len(body) <= ChatBatcherMax {
 		return p.Translate(be, body, scratch)
 	}
 	switch cfg.schema {
-	case C.AIGW_SCHEMA_OPENAI, C.AIGW_SCHEMA_AZURE_OPENAI, C.AIGW_SCHEMA_AWS_BEDROCK, C.AIGW_SCHEMA_GCP_ANTHROPIC, C.AIGW_SCHEMA_AWS_ANTHROPIC:
+	case C.AIGW_SCHEMA_OPENAI, C.AIGW_SCHEMA_AZURE_OPENAI, C.AIGW_SCHEMA_AWS_BEDROCK, C.AIGW_SCHEMA_GCP_ANTHROPIC, C.AIGW_SCHEMA_AWS_ANTHROPIC,
+		C.AIGW_SCHEMA_GCP_VERTEX:
 	default:
 		return p.Translate(be, body, scratch)
 	}
@@ -181,6 +184,8 @@ func (p *Pipeline) TranslateChat(be Backend, cfg *C.aigw_backend_cfg, body, scra
 		rc = C.aigw_chat_bedrock_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out)
 	case C.AIGW_SCHEMA_GCP_ANTHROPIC, C.AIGW_SCHEMA_AWS_ANTHROPIC:
 		rc = C.aigw_chat_anthropic_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out)
+	case C.AIGW_SCHEMA_GCP_VERTEX:
+		rc = C.aigw_chat_gemini_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out)
 	default:
 		rc = C.aigw_chat_translate_large_host(p.bulk, cfg, (*C.uint8_t)(unsafe.Pointer(&body[0])), &off, &ln, 1, &out)
 	}

@@ -4,7 +4,8 @@ include_usage, Azure, and AWS Bedrock with and without an override, also on the 
 single-request wall latency at 128 KiB, 1 MiB and 4 MiB, and the serial walk's worst cases.  The same for
 aigw_chat_anthropic_translate_large_* (GCP Vertex AI and AWS Bedrock) on the Anthropic-shaped transcripts of
 tests/test_chat_anthropic_large_cpu.py, whose "tools" the Anthropic plan declines in the agent transcripts (`--only anthropic`
-runs that part alone).  Prints one JSON line per measurement, each with the card's
+runs that part alone), and for aigw_chat_gemini_translate_large_* on the long-context requests of
+tests/test_chat_gemini_large_cpu.py (`--only gemini`).  Prints one JSON line per measurement, each with the card's
 name and power limit read in the same run.  Needs an H100; there is no CPU path."""
 import json
 import os
@@ -101,6 +102,7 @@ def main():
         emit(what="serial_walk_worst_case", layout=label, bytes=len(b), ms=round(ms, 1), status=int(g["status"]), reason=int(g["reason"]))
     bedrock(ctx, corpus)
     anthropic(ctx)
+    gemini(ctx)
     ctx.close()
 
 
@@ -195,6 +197,55 @@ def anthropic(ctx):
         emit(what="serial_walk_worst_case", target="gcp_anthropic", layout=label, bytes=len(b), ms=round(ms, 1), status=int(g["status"]), reason=int(g["reason"]))
 
 
+def gemini(ctx):
+    import aigw_b200 as A
+    import test_chat_gemini_large_cpu as GM
+    import test_chat_gemini_large_gpu as GG
+    dev = "chat_gemini_translate_large_device"
+    rng = np.random.default_rng(1234)
+    corpus = [GM.gemini_chat(900 + i, int(np.exp(rng.uniform(np.log(64 << 10), np.log(8 << 20))))) for i in range(18)]
+    subset = [b for b in corpus if not GM.json_schema_side(json.loads(b)["model"])]
+    for name, bodies, override in (("gemini", corpus, None), ("gemini_override", subset, GM.OVERRIDE)):
+        c = ctx.cfg("gcp-vertexai", model_override=override)
+        got = ctx.chat_gemini_translate_large(c, bodies)
+        assert all(g["status"] == A.AIGW_OK for g in got), [(g["status"], g["reason"]) for g in got]
+        ms, used = device_call(ctx, c, bodies, fn=dev, k=3)
+        nbytes = sum(map(len, bodies))
+        emit(what="device_call", target=name, requests=len(bodies), request_bytes=nbytes, output_bytes=used, ms=round(ms, 3),
+             gb_per_s_in=round(nbytes / ms / 1e6, 2), max_len=max(map(len, bodies)))
+        arena, offs, lens = A.pack_bodies(bodies)
+        ctx.chat_gemini_translate_large_host(c, arena, offs, lens)
+        t = []
+        for _ in range(5):
+            t0 = time.perf_counter(); ctx.chat_gemini_translate_large_host(c, arena, offs, lens); t.append(time.perf_counter() - t0)
+        emit(what="host_call", target=name, ms=round(1e3 * float(np.median(t)), 2), gb_per_s_in=round(nbytes / float(np.median(t)) / 1e9, 2))
+    c = ctx.cfg("gcp-vertexai")
+    for size in (128 << 10, 1 << 20, 4 << 20):
+        b = GM.gemini_chat(77, size)
+        arena, offs, lens = A.pack_bodies([b])
+        assert ctx.chat_gemini_translate_large(c, [b])[0]["status"] == A.AIGW_OK
+        t = []
+        for i in range(60):
+            t0 = time.perf_counter(); ctx.chat_gemini_translate_large_host(c, arena, offs, lens); t.append(time.perf_counter() - t0)
+        t = np.array(t[10:]) * 1e6
+        ms, _ = device_call(ctx, c, [b], reps=10, fn=dev, k=3)
+        emit(what="single_request_wall_us", target="gemini", bytes=len(b), p50=round(float(np.percentile(t, 50))), p99=round(float(np.percentile(t, 99))), kernel_ms=round(ms, 3))
+    # the serial walk's worst cases at 16 MiB - 1: one-word user messages (one merged content), alternating one-word user and
+    # assistant messages, and one-word user messages after a "tools" array that sits at the key-order work budget
+    n = (16 << 20) - 1
+    users = '{"model":"m","messages":[' + ",".join(['{"role":"user","content":"x"}'] * ((n - 64) // 30)) + "]}"
+    alt = '{"model":"m","messages":[' + ",".join(['{"role":"user","content":"x"},{"role":"assistant","content":"x"}'] * ((n - 64) // 66)) + "]}"
+    at_budget = GG.budget_bodies()[0]
+    tools = at_budget[:-1].decode() + ',"messages":[' + ",".join(['{"role":"user","content":"x"}'] * ((n - 64 - len(at_budget)) // 30)) + "]}"
+    tools = tools.replace('"messages": [{"role": "user", "content": "hi"}], ', "", 1)
+    for label, s in (("one_word_user_messages", users), ("alternating_user_assistant", alt), ("tools_at_work_budget", tools)):
+        b = s.encode()
+        b = b + b" " * (n - len(b))
+        ms, _ = device_call(ctx, c, [b], reps=3, fn=dev, k=3)
+        g = ctx.chat_gemini_translate_large(c, [b])[0]
+        emit(what="serial_walk_worst_case", target="gemini", layout=label, bytes=len(b), ms=round(ms, 1), status=int(g["status"]), reason=int(g["reason"]))
+
+
 CARD = "unknown"
 if __name__ == "__main__":
     CARD = card()
@@ -202,6 +253,11 @@ if __name__ == "__main__":
         import aigw_b200 as A
         ctx = A.Context(0)
         anthropic(ctx)
+        ctx.close()
+    elif sys.argv[1:] == ["--only", "gemini"]:
+        import aigw_b200 as A
+        ctx = A.Context(0)
+        gemini(ctx)
         ctx.close()
     else:
         main()
