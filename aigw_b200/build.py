@@ -25,9 +25,11 @@ GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 #     VIADD R21, R21, 0x1 ; IMAD.WIDE.U32 R8, R21, 0x10, R52 ; LD.E.128 R8, desc[UR8][R8.64]     (R52: the ops base, offset +0)
 # so it stays at -O3 as well.  chat_gemini_large_kernel.cu runs that emit too, and its -O3 SASS also reloads ops[k]:
 #     VIADD R21, R21, 0x1 ; IMAD.WIDE.U32 R2, R21, 0x10, R48 ; LD.E.128 R8, desc[UR8][R2.64]     (R48: the ops base, offset +0)
+# so it stays at -O3.  messages_large_kernel.cu runs that emit too, and its -O3 SASS also reloads ops[k]:
+#     VIADD R21, R21, 0x1 ; IMAD.WIDE.U32 R2, R21, 0x10, R52 ; LD.E.128 R8, desc[UR8][R2.64]     (R52: the ops base, offset +0)
 # so it stays at -O3.
 PTXAS = {"chat_small_g11.cu": ["-Xptxas", "-O1"], "chat_small_g12.cu": ["-Xptxas", "-O1"]}
-SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_walk_g10.cu", "chat_walk_g11.cu", "chat_walk_g12.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "chat_small_g10.cu", "chat_small_g11.cu", "chat_small_g12.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "rerank_large_kernel.cu", "emb_large_kernel.cu", "chat_large_kernel.cu", "chat_large_record.cu", "chat_bedrock_large_kernel.cu", "chat_anthropic_large_kernel.cu", "chat_gemini_large_kernel.cu", "responses_large_kernel.cu", "completions_large_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
+SOURCES = ["lib.cu", "chat_kernel.cu", "chat_walk.cu", "chat_walk_g0.cu", "chat_walk_g1.cu", "chat_walk_g2.cu", "chat_walk_g3.cu", "chat_walk_g4.cu", "chat_walk_g5.cu", "chat_walk_g6.cu", "chat_walk_g7.cu", "chat_walk_g8.cu", "chat_walk_g9.cu", "chat_walk_g10.cu", "chat_walk_g11.cu", "chat_walk_g12.cu", "chat_small_g0.cu", "chat_small_g1.cu", "chat_small_g2.cu", "chat_small_g3.cu", "chat_small_g4.cu", "chat_small_g5.cu", "chat_small_g6.cu", "chat_small_g7.cu", "chat_small_g8.cu", "chat_small_g9.cu", "chat_small_g10.cu", "chat_small_g11.cu", "chat_small_g12.cu", "sse_kernel.cu", "bedrock_stream_kernel.cu", "stream_kernel.cu", "bpe_kernel.cu", "emb_kernel.cu", "rerank_large_kernel.cu", "emb_large_kernel.cu", "chat_large_kernel.cu", "chat_large_record.cu", "chat_bedrock_large_kernel.cu", "chat_anthropic_large_kernel.cu", "chat_gemini_large_kernel.cu", "messages_large_kernel.cu", "responses_large_kernel.cu", "completions_large_kernel.cu", "mutate_kernel.cu", "batcher.cu", "sha256_kernel.cu", "cel_kernel.cu"]
 
 
 def nvcc():

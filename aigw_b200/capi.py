@@ -44,7 +44,7 @@ assert MutResult.itemsize == 16
 EXPORTS = ["aigw_bind_numa", "aigw_stream_open", "aigw_stream_open_batch", "aigw_stream_chunks", "aigw_stream_chunks_soa", "aigw_stream_chunk", "aigw_stream_close", "aigw_stream_close_batch",
            "aigw_version", "aigw_init", "aigw_destroy", "aigw_last_error", "aigw_device_sm_count", "aigw_host_alloc", "aigw_host_free",
            "aigw_device_alloc", "aigw_device_free", "aigw_memcpy_h2d", "aigw_memcpy_d2h", "aigw_memset_d", "aigw_sync",
-           "aigw_chat_translate_device", "aigw_chat_translate_device_mapped", "aigw_chat_last_profile", "aigw_chat_set_profile", "aigw_chat_set_small_batch", "aigw_chat_translate_host", "aigw_rerank_translate_large_device", "aigw_rerank_translate_large_host", "aigw_embeddings_translate_large_device", "aigw_embeddings_translate_large_host", "aigw_chat_translate_large_device", "aigw_chat_translate_large_host", "aigw_chat_bedrock_translate_large_device", "aigw_chat_bedrock_translate_large_host", "aigw_chat_anthropic_translate_large_device", "aigw_chat_anthropic_translate_large_host", "aigw_chat_gemini_translate_large_device", "aigw_chat_gemini_translate_large_host", "aigw_sse_usage_device", "aigw_sse_usage_host", "aigw_response_usage_device", "aigw_response_usage_host", "aigw_embeddings_response_usage_device", "aigw_embeddings_response_usage_host", "aigw_completions_response_usage_device", "aigw_completions_response_usage_host", "aigw_responses_response_usage_device", "aigw_responses_response_usage_host", "aigw_rerank_response_usage_device", "aigw_rerank_response_usage_host", "aigw_usage_costs_device",
+           "aigw_chat_translate_device", "aigw_chat_translate_device_mapped", "aigw_chat_last_profile", "aigw_chat_set_profile", "aigw_chat_set_small_batch", "aigw_chat_translate_host", "aigw_rerank_translate_large_device", "aigw_rerank_translate_large_host", "aigw_embeddings_translate_large_device", "aigw_embeddings_translate_large_host", "aigw_chat_translate_large_device", "aigw_chat_translate_large_host", "aigw_chat_bedrock_translate_large_device", "aigw_chat_bedrock_translate_large_host", "aigw_chat_anthropic_translate_large_device", "aigw_chat_anthropic_translate_large_host", "aigw_chat_gemini_translate_large_device", "aigw_chat_gemini_translate_large_host", "aigw_messages_translate_large_device", "aigw_messages_translate_large_host", "aigw_sse_usage_device", "aigw_sse_usage_host", "aigw_response_usage_device", "aigw_response_usage_host", "aigw_embeddings_response_usage_device", "aigw_embeddings_response_usage_host", "aigw_completions_response_usage_device", "aigw_completions_response_usage_host", "aigw_responses_response_usage_device", "aigw_responses_response_usage_host", "aigw_rerank_response_usage_device", "aigw_rerank_response_usage_host", "aigw_usage_costs_device",
            "aigw_bedrock_stream_device", "aigw_bedrock_stream_host", "aigw_body_mutate_device", "aigw_body_mutate_host",
            "aigw_cost_compile", "aigw_cost_program_free", "aigw_usage_costs_cel_device", "aigw_usage_costs_cel_host", "aigw_sha256_device", "aigw_chat_body_sha256_device", "aigw_sha256_host", "aigw_bpe_load", "aigw_bpe_free", "aigw_bpe_count_device", "aigw_bpe_count_host", "aigw_embeddings_count_device", "aigw_embeddings_count_host", "aigw_batcher_start", "aigw_batcher_add_backend", "aigw_batcher_translate", "aigw_batcher_translate_to", "aigw_batcher_get_stats", "aigw_batcher_stop"]
 
@@ -132,6 +132,8 @@ def load_library():
     L.aigw_chat_anthropic_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
     L.aigw_chat_gemini_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
     L.aigw_chat_gemini_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
+    L.aigw_messages_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
+    L.aigw_messages_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
     L.aigw_responses_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
     L.aigw_responses_translate_large_host.argtypes = L.aigw_chat_translate_host.argtypes
     L.aigw_completions_translate_large_device.argtypes = L.aigw_chat_translate_device.argtypes
@@ -375,6 +377,24 @@ class Context:
         ms = C.c_float(0)
         self._check(self.L.aigw_chat_gemini_translate_large_device(self.h, C.byref(cfg), d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used,
                                                                    None, C.byref(ms) if timed else None), "chat_gemini_translate_large_device")
+        return ms.value
+
+    # ---- /v1/messages requests of any size below 16 MiB to OpenAI and AWS Bedrock Converse (one CTA streams one request)
+    def messages_translate_large_host(self, cfg, arena, offs, lens):
+        """Same results as chat_translate_host under AIGW_SCHEMA_MSG_OPENAI / AIGW_SCHEMA_MSG_AWS_BEDROCK, for bodies of 1 byte to
+        16 MiB - 1."""
+        return self._translate_host(self.L.aigw_messages_translate_large_host, "messages_translate_large_host", cfg, arena, offs, lens)
+
+    def messages_translate_large(self, cfg, bodies):
+        """list of bytes → the same dicts as chat_translate"""
+        arena, offs, lens = pack_bodies(bodies)
+        res, out, _ = self.messages_translate_large_host(cfg, arena, offs, lens)
+        return self._records(bodies, res, out)
+
+    def messages_translate_large_device(self, cfg, d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used, timed=True):
+        ms = C.c_float(0)
+        self._check(self.L.aigw_messages_translate_large_device(self.h, C.byref(cfg), d_bodies, d_offs, d_lens, n, max_len, d_out, out_cap, d_res, d_used,
+                                                                None, C.byref(ms) if timed else None), "messages_translate_large_device")
         return ms.value
 
     # ---- /v1/responses requests of any size below 16 MiB (one CTA streams one request)

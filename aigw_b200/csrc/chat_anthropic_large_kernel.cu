@@ -213,7 +213,7 @@ __device__ __forceinline__ void an_tool_result(RecWalk& W, const RecWalk::Msg& t
 }
 
 // plan_anthropic after ParseBody's top-level checks
-struct AnPlan {
+struct AnPlan : ClChatTop {
   static __device__ __forceinline__ void plan(const ChatLargeParams& P, ClShared& S, RecWalk& W, const RecWalk::Top& t, bool stream) {
     const LDoc& d = W.d;
     const bool gcp = P.gcp != 0;

@@ -15,7 +15,7 @@ namespace {
 
 // plan_bedrock after ParseBody's top-level checks: ":path" /model/{PathEscape(model or override)}/converse[-stream], then the
 // Converse body
-struct BlPlan {
+struct BlPlan : ClChatTop {
   static __device__ __forceinline__ void plan(const ChatLargeParams& P, ClShared& S, RecWalk& W, const RecWalk::Top& t, bool stream) {
     if (!W.bad()) {
       W.lit(L_PATH_MODEL);

@@ -132,7 +132,7 @@ __device__ __forceinline__ bool gem_system(RecWalk& W, const RecWalk::Msg& g, bo
 }
 
 // plan_gemini after ParseBody's top-level checks
-struct GemPlan {
+struct GemPlan : ClChatTop {
   static __device__ __forceinline__ void plan(const ChatLargeParams& P, ClShared& S, RecWalk& W, const RecWalk::Top& t, bool stream) {
     const LDoc& d = W.d;
     if (W.bad()) return;

@@ -39,6 +39,7 @@ struct ChatLargeParams {
   char lits[512];
   uint32_t max_len;           // the call's longest request (the record kernels of chat_large_record.cuh: the slice's layout)
   uint32_t gcp;               // chat_anthropic_large_kernel: AIGW_SCHEMA_GCP_ANTHROPIC, else AIGW_SCHEMA_AWS_ANTHROPIC
+  uint32_t bedrock;           // messages_large_kernel: AIGW_SCHEMA_MSG_AWS_BEDROCK, else AIGW_SCHEMA_MSG_OPENAI
 };
 
 static constexpr uint32_t kChatLargeMaxDepth = 48;

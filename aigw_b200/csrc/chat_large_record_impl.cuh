@@ -1,7 +1,7 @@
 // The record phase of the large-request chat kernels that rebuild the body (chat_bedrock_large_kernel.cu,
 // chat_anthropic_large_kernel.cu), after the scan and depth pass of large_request.cuh:
 //   grammar   thread 0 checks the token grammar and writes the jump table
-//   walk      thread 0 runs scan_top and the kernel's planner over the emitting walk (ClWalkT<ClOut>, chat_bedrock_walk.cuh): its
+//   walk      thread 0 runs the planner's top-level scan and the planner over the emitting walk (ClWalkT<ClOut>, chat_bedrock_walk.cuh): its
 //             checks in the translate pass's order, and the record as copy ops in the CTA's slice.  A string with an escape the
 //             encoder re-spells (\/ \b \f \u) keeps its other stretches as body spans, its re-spelled runs go into scratch; a tool
 //             call's "arguments" are unescaped, checked and re-serialised into scratch.
@@ -10,9 +10,12 @@
 // The emit differs from emb_large_kernel's, whose cursor also walks escape entries inside its string ops; this record has none.
 //
 // A kernel is cl_request_loop<ClRecordRequest<Plan>>, where Plan has
-//   static void plan(const ChatLargeParams&, ClShared&, RecWalk& W, const RecWalk::Top& t, bool stream)
-// called by thread 0 after scan_top has passed, with the model span, the stream flag and body_kind already set: it records the
-// ":path" (and sets S.path_len), then the body, or declines through W.
+//   using Top = …                                  the top-level members its scan keeps, with `model` and `stream` (value tokens,
+//                                                  kNone when absent or null)
+//   static bool scan(RecWalk& W, Top& t)           the top-level scan: true when it passed (the chat planners: ClChatTop, scan_top)
+//   static void plan(const ChatLargeParams&, ClShared&, RecWalk& W, const Top& t, bool stream)
+// plan is called by thread 0 after the scan has passed, with the model span, the stream flag and body_kind already set: it records
+// the ":path" (and sets S.path_len), then the body, or declines through W.
 #pragma once
 #include "chat_bedrock_walk.cuh"
 #include "chat_large_record.cuh"
@@ -62,13 +65,14 @@ struct ClOut {
   // a re-spelled byte run into scratch: room for `need` more bytes
   __device__ bool room(uint32_t need) { if (rs_n + need > rs_cap) { err = AIGW_R_SCRATCH; return false; } return true; }
 
-  // emit_str / emit_str_respelled of a body string v, quotes included.  The scan has checked every \u escape's hex digits and
-  // declined lone surrogates, so every escape here decodes.
-  __device__ void str(const LDoc& d, uint32_t v) {
+  // emit_str / emit_str_respelled of a body string v, quotes included (kInner: without them).  The scan has checked every \u
+  // escape's hex digits and declined lone surrogates, so every escape here decodes.
+  template <bool kInner>
+  __device__ __forceinline__ void str_q(const LDoc& d, uint32_t v) {
     const uint32_t q0 = d.tok(v), q1 = d.tok(v + 1);
-    if (!d.str_nc(v)) { push(REC_BODY, q0, q1 + 1u - q0); return; }
+    if (!d.str_nc(v)) { push(REC_BODY, kInner ? q0 + 1u : q0, kInner ? q1 - q0 - 1u : q1 + 1u - q0); return; }
     const uint8_t* s = d.s;
-    uint32_t seg = q0, i = q0 + 1, run = 0;
+    uint32_t seg = kInner ? q0 + 1u : q0, i = q0 + 1, run = 0;
     bool in_run = false;
     while (i < q1) {
       const uint32_t c = s[i];
@@ -100,8 +104,11 @@ struct ClOut {
       rs_n += w; i += used;
     }
     if (in_run) { push(REC_SCR, run, rs_n - run); seg = q1; }
-    push(REC_BODY, seg, q1 + 1u - seg);
+    push(REC_BODY, seg, (kInner ? q1 : q1 + 1u) - seg);
   }
+  __device__ void str(const LDoc& d, uint32_t v) { str_q<false>(d, v); }
+  // emit_str_inner: the string's bytes as the encoder spells them, without the quotes (text blocks concatenated into one string)
+  __device__ void str_inner(const LDoc& d, uint32_t v) { str_q<true>(d, v); }
 };
 
 using RecWalk = ClWalkT<ClOut>;
@@ -117,8 +124,8 @@ __device__ __forceinline__ RecSlice rec_carve(uint2* rest, uint32_t max_len) {
 
 // The model of the ":path" (the override, or the request's model): url.PathEscape'd (kEscape) or raw.  A model that needs no
 // escaping is a body span; an escaped one, or the override, goes into scratch.
-template <bool kEscape>
-__device__ __forceinline__ void rec_path_model(const ChatLargeParams& P, const ClShared& S, RecWalk& W, const RecWalk::Top& t) {
+template <bool kEscape, class Top = RecWalk::Top>
+__device__ __forceinline__ void rec_path_model(const ChatLargeParams& P, const ClShared& S, RecWalk& W, const Top& t) {
   const LDoc& d = W.d;
   const bool ov = P.override_len != 0;
   const uint8_t* mp = ov ? S.lits + S.lit_off[CL_OVERRIDE] : t.model != kNone ? d.s + d.str_off(t.model) : nullptr;
@@ -157,6 +164,12 @@ __device__ __forceinline__ unsigned long long rec_excl(unsigned long long v, uns
   return pre + incl - v;
 }
 
+// the top-level scan of the /v1/chat/completions planners: ParseBody's checks (scan_top)
+struct ClChatTop {
+  using Top = RecWalk::Top;
+  static __device__ __forceinline__ bool scan(RecWalk& W, Top& t) { return W.scan_top(t); }
+};
+
 template <class Plan>
 struct ClRecordRequest {
   using Scratch = uint2*;
@@ -186,8 +199,8 @@ struct ClRecordRequest {
         if (vr) f = vr == AIGW_R_SYNTAX ? AIGW_R_E400_SYNTAX : vr;
       }
       if (!f) {
-        RecWalk::Top t;
-        if (W.scan_top(t)) {
+        typename Plan::Top t;
+        if (Plan::scan(W, t)) {
           const bool stream = t.stream != kNone && W.d.ty(t.stream) == 't';
           if (t.model != kNone) {
             const uint32_t ml = W.d.str_len(t.model);

@@ -29,6 +29,7 @@
 #include "chat_bedrock_large_kernel.cuh"
 #include "chat_anthropic_large_kernel.cuh"
 #include "chat_gemini_large_kernel.cuh"
+#include "messages_large_kernel.cuh"
 #include "responses_large_kernel.cuh"
 #include "completions_large_kernel.cuh"
 
@@ -116,9 +117,10 @@ struct aigw_ctx {
   Scratch<uint8_t> d_cl_ws;
   // large chat requests to AWS Bedrock (aigw_chat_bedrock_translate_large_device): chat_large's slice, then ops and scratch
   Scratch<uint8_t> d_bl_ws;
-  // large chat requests to Anthropic on GCP Vertex AI / AWS Bedrock (aigw_chat_anthropic_translate_large_device) and to Gemini on
-  // GCP Vertex AI (aigw_chat_gemini_translate_large_device): the same slice layout.  The two calls share it, as one device call is
-  // in flight per context; a second grow-only workspace would double the device memory held (about 1 GB at 128 KiB bodies).
+  // large chat requests to Anthropic on GCP Vertex AI / AWS Bedrock (aigw_chat_anthropic_translate_large_device), to Gemini on
+  // GCP Vertex AI (aigw_chat_gemini_translate_large_device) and large /v1/messages requests to OpenAI / AWS Bedrock Converse
+  // (aigw_messages_translate_large_device): the same slice layout.  The three calls share it, as one device call is in flight per
+  // context; another grow-only workspace would hold up to 1 GiB more device memory (about 1 GB at 128 KiB bodies).
   Scratch<uint8_t> d_al_ws;
   // large /v1/responses requests (aigw_responses_translate_large_device): one workspace slice per CTA (tokens, jump table, escape counts)
   Scratch<uint8_t> d_rl_ws;
@@ -1179,6 +1181,41 @@ int aigw_chat_gemini_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg*
                                           const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
   // the densest record is a user text of backslash-b escapes (two bytes each, re-spelled as six-byte u-escapes): 3.0 times the body
   return large_host_retry(aigw_chat_gemini_translate_large_device, "aigw_chat_gemini_translate_large_host", 3, ctx, cfg, bodies, offsets, lens, n, out);
+}
+
+// ------------------------------------------------------------------ /v1/messages to OpenAI and AWS Bedrock Converse of any size below 16 MiB
+int aigw_messages_translate_large_device(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* d_bodies, const uint64_t* d_offsets,
+                                         const uint32_t* d_lens, uint32_t n, uint32_t max_len, uint8_t* d_out, uint64_t out_capacity,
+                                         aigw_doc_result* d_results, uint64_t* d_out_used, void* stream, float* kernel_ms) {
+  if (!ctx) return -2;
+  if (n == 0) { if (kernel_ms) *kernel_ms = 0; return 0; }
+  ENTER_ON(stream);
+  ChatParams C;
+  fill_params(C, cfg);   // the ":path" prefix and the override exactly as the translate pass gets them
+  const int32_t schema = cfg ? cfg->schema : -1;
+  ChatLargeParams P;
+  P.bodies = d_bodies; P.offsets = d_offsets; P.lens = d_lens; P.n = n; P.results = d_results;
+  P.out = d_out; P.out_capacity = out_capacity; P.out_used = (unsigned long long*)d_out_used;
+  P.call_reason = schema == AIGW_SCHEMA_MSG_OPENAI || schema == AIGW_SCHEMA_MSG_AWS_BEDROCK ? 0u : (uint32_t)AIGW_R_SCHEMA;
+  P.bedrock = schema == AIGW_SCHEMA_MSG_AWS_BEDROCK ? 1u : 0u;
+  P.gcp = 0; P.azure = 0; P.cost_configured = 0; P.force_mutation = 0; P.override_ok = 1;   // the body is always rebuilt
+  P.override_len = C.override_len;
+  chat_large_lits(P, C.openai_path, C.prefix_len, C.override_model, C.override_len, C.api_version, C.version_len);
+  const uint32_t ml = max_len && max_len < (1u << 24) ? max_len : (1u << 24) - 1u;
+  P.max_len = ml;
+  P.tok_cap = chat_large_tok_cap(ml);
+  P.slice = chat_record_large_slice_bytes(ml);
+  const int grid = chat_record_large_grid(ctx->sm_count, ml);
+  CK(ctx->d_al_ws.ensure((size_t)grid * P.slice));
+  P.ws = ctx->d_al_ws;
+  if (int rc = take_counters(ctx, 1, st, &P.next)) return rc;
+  return timed(ctx, st, kernel_ms, [&] { CK(launch_messages_large(P, grid, st)); return 0; });
+}
+
+int aigw_messages_translate_large_host(aigw_ctx* ctx, const aigw_backend_cfg* cfg, const uint8_t* bodies, const uint64_t* offsets,
+                                       const uint32_t* lens, uint32_t n, aigw_batch_out* out) {
+  // the densest record is a text of backslash-b escapes (two bytes each, re-spelled as six-byte u-escapes): 3.0 times the body
+  return large_host_retry(aigw_messages_translate_large_device, "aigw_messages_translate_large_host", 3, ctx, cfg, bodies, offsets, lens, n, out);
 }
 
 // ------------------------------------------------------------------ /v1/responses and /v1/completions requests of any size below 16 MiB
